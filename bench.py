@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""Benchmark of the B200-native PIN-SLAM hot path (contract: see the task statement / DESIGN.md §4).
+"""Benchmark of the H100-native (sm_90a) PIN-SLAM hot path (DESIGN.md §4).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 Workload at N=1: BASELINE.json configs[1] -- the fused kNN + SDF-MLP query (K1) over a batch of
 200 000 query points, K=8 neighbours, 32-d features, 2x64 decoder, C=33 probe cells, with the
@@ -24,6 +24,9 @@ analytic d sdf / d x.  One *step* is one pass of the hot path over that batch.
             next to the reference's own Tracker/Mapper in PyTorch-CUDA mode
 N>1: the query path has no exchange step -- every rank runs the same per-GPU batch on its own map
 replica (weak scaling); no collective on the data path.
+
+--dump-outputs DIR writes what the last timed step computed (the arrays NeuralPoints.query_sdf returns: sdf, grad,
+sdf_std, nn_count, certainty) as DIR/<name>.npy; the workload is seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -37,7 +40,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 N_QUERY = 200_000
-FALLBACK_HBM_GBS = 6650.0
+FALLBACK_HBM_GBS = 3350.0
 
 
 def hbm_peak():
@@ -47,7 +50,7 @@ def hbm_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return FALLBACK_HBM_GBS, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return FALLBACK_HBM_GBS, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 def ncu_traffic():
@@ -396,6 +399,21 @@ def mapper_benchmark(args, standalone=True):
     return res
 
 
+def dump_outputs(res, directory):
+    """The arrays of one query_sdf result as <directory>/<name>.npy: floating arrays as float32 (float64 stays float64),
+    integer arrays (nn_count) as float64.  Entries named _* are the call's scratch buffers, not results."""
+    import numpy as np
+    import torch
+
+    os.makedirs(directory, exist_ok=True)
+    for name, v in sorted(res.items()):
+        if name.startswith("_") or not isinstance(v, torch.Tensor):
+            continue
+        a = v.detach().cpu()
+        a = a.double() if (not a.is_floating_point() or a.dtype == torch.float64) else a.float()
+        np.save(os.path.join(directory, name + ".npy"), a.numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -412,7 +430,11 @@ def main():
                          "configuration every committed number refers to")
     ap.add_argument("--workload", default="query", choices=["query", "mapper"],
                     help="query = BASELINE configs[1] (default, the headline); mapper = configs[4] data-parallel training")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="query workload: write the outputs of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     global MAP_SCALE
     MAP_SCALE = float(args.map_scale)
@@ -478,6 +500,8 @@ def main():
     launches = ops.launch_count() - launches0
     total_ms = sum(step_ms)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(out, args.dump_outputs)
 
     # ---- end to end through the public call with host buffers
     q_host = q.cpu().pin_memory()
@@ -534,7 +558,7 @@ def main():
                          "traffic": ncu_traffic(), "peak_source": peak_src, "kernel": k1_kernels,
                          "kernel_ms_median": kernel_ms,
                          "note": "K1 = the two launches of the query pipeline (neighbour search, then the warp-specialised "
-                                 "gather + tcgen05 decoder with forward-mode d/dq); achieved = algorithmic bytes/query x "
+                                 "gather + wgmma decoder with forward-mode d/dq); achieved = algorithmic bytes/query x "
                                  "queries / mean CUDA-event time of the "
                                  "pipeline; traffic = dram bytes of both launches (ncu, profiles/k1_traffic.json)"},
             "clocks": clocks,
@@ -561,7 +585,7 @@ def main():
                 fn = lambda: vnpm.query_sdf(vq, vdec, need_grad=True, out=vo)  # noqa: E731
                 for _ in range(3):
                     fn()
-                ms = sorted(time_k1(fn, 8))[4]
+                ms = sorted(time_k1(fn, args.steps))[args.steps // 2]
                 vn_occ, vk_v, _ = workload_stats(vnpm, vq, k)
                 vbq = bytes_per_query(vnpm.neighbor_K, vn_occ, vk_v, vcfg.feature_dim)
                 ach = vbq * N_QUERY / (ms * 1e-3) / 1e9
@@ -573,7 +597,7 @@ def main():
                     # dense [N*K, D] x [D, 64] x [64, 64] chain, forward + backward to the input: 2 flops per MAC
                     D, H = vcfg.feature_dim + 3, 64
                     flops = 2.0 * (D * H + H * H + H) * k * 2 * N_QUERY
-                    sm_peak = 148 * 128 * 2 * 1.965e9 / 1e12  # fp32 SIMT FMA peak of this part (TFLOP/s)
+                    sm_peak = 132 * 128 * 2 * 1.98e9 / 1e12  # fp32 SIMT FMA peak of an H100 SXM (TFLOP/s, data sheet)
                     v["compute_roofline"] = {"bound": "fp32 (3xTF32 on tensor cores counts as fp32 work)",
                                              "achieved": flops / (ms * 1e-3) / 1e12, "peak": sm_peak, "unit": "TFLOP/s",
                                              "frac": flops / (ms * 1e-3) / 1e12 / sm_peak}
@@ -591,7 +615,7 @@ def main():
         del flush
         torch.cuda.empty_cache()
         try:
-            md = mapper_benchmark(argparse.Namespace(steps=max(20, args.steps), warmup=args.warmup), standalone=False)
+            md = mapper_benchmark(argparse.Namespace(steps=args.steps, warmup=args.warmup), standalone=False)
             if line is not None:
                 line["mapper_dp"] = {"ms_per_iter": md["ms_per_step"], "samples_per_s": md["value"],
                                      "allreduce_bytes": 4 * md["config"]["allreduce_floats"],
@@ -620,7 +644,7 @@ def main():
                 line["reference_cuda_baseline"] = {
                     "value": bq * g["queries_per_s"] / 1e9, "unit": "GB/s", "ms_per_step": g["s_per_step"] * 1e3,
                     "what": "unmodified reference Tracker.query_source_points (oracle/_ref) in PyTorch-CUDA mode on this "
-                            "B200, all 200k queries per step"}
+                            "GPU, all 200k queries per step"}
                 line["speedup_vs_reference_cuda"] = g["s_per_step"] * 1e3 / ms_per_step
             else:
                 line["reference_cuda_baseline"] = g

@@ -1,5 +1,5 @@
 /*
- * pinb200.h -- C ABI of the B200-native (sm_100a) PIN-SLAM hot path.
+ * pinb200.h -- C ABI of the H100-native (sm_90a) PIN-SLAM hot path.
  *
  * The reference (PRBonn/PIN_SLAM) is 100 % Python/PyTorch and has no native
  * boundary of its own; the boundary it *does* have for this path is the Python
@@ -72,7 +72,7 @@ typedef struct pinb200_map_view {
   int32_t cur_ts;
   float diff_travel_dist_local;
   int32_t after_pgo;           /* rotate neighbour vectors by the point quaternion (:645) */
-  /* Probe index (B200 layout, built by pinb200_build_probe_index): a succinct rank structure holding the ANSWERS
+  /* Probe index (built by pinb200_build_probe_index): a succinct rank structure holding the ANSWERS
    * of the hash table in L2-resident form.  A probe of the fused query reads one 8-byte word and, on a hit, one
    * 16-byte record, both from arrays of a few MB, instead of walking buffer_pt_index -> neural_points /
    * point_ts_create -> travel_dist / global2local (model/neural_points.py:963-999,573) in a table of several
@@ -118,27 +118,27 @@ typedef struct pinb200_query_opts {
   const double* transform;  /* optional device ptr, 4x4 row-major fp64: q = T*p evaluated in fp32 (tools.py:534-553) */
   void* workspace;          /* optional device scratch of >= pinb200_query_workspace_bytes(N) bytes.  With it, batches
                                of >= PINB200_SPLIT_MIN_QUERIES (weighted_first: _WF) queries run as two launches (neighbour search at high
-                               occupancy, then gather + decoder on tcgen05 tiles); without it, or for small batches,
+                               occupancy, then gather + decoder on wgmma tiles); without it, or for small batches,
                                one fused launch.  The neighbour search is bit-identical either way; the decoder
                                outputs agree within the 3xTF32 bound (different accumulation order). */
   int64_t workspace_bytes;
 } pinb200_query_opts;
 
 #define PINB200_SPLIT_MIN_QUERIES 32768   /* decode-every-neighbour maps */
-#define PINB200_SPLIT_MIN_QUERIES_WF 1024 /* weighted_first maps whose decoder runs on the tcgen05 kernels (hidden 64, 1-2 layers,
+#define PINB200_SPLIT_MIN_QUERIES_WF 1024 /* weighted_first maps whose decoder runs on the wgmma kernels (hidden 64, 1-2 layers,
                                              F in {8,16,32}): the two-launch pipeline is faster from ~1 k queries on */
 int64_t pinb200_query_workspace_bytes(int64_t n_queries);
 /* Run-time tunables of the query path (process-wide; for tests and A/B measurements):
      "split_min_queries"  batch size from which the two-launch pipeline is used, both kinds of map (<= 0 restores the
                           defaults PINB200_SPLIT_MIN_QUERIES / PINB200_SPLIT_MIN_QUERIES_WF)
      "split_min_queries_wf"  the same for weighted_first maps only
-     "decode_variant"     0: phase-synchronous tcgen05 decode with backward MMAs (decode_umma_kernel)
+     "decode_variant"     0: phase-synchronous wgmma decode with backward MMAs (decode_umma_kernel)
                           1: warp-specialised forward-mode decode (wsq_decode_kernel; default)
      "ws_profile"         1: wsq_decode_kernel records per-warp phase cycle counters (pinb200_debug_read)
    The reference has no equivalent: its decode is model/decoder.py:61-85 + autograd (utils/tools.py:247-260). */
 int pinb200_set_option(const char* name, int64_t value);
 /* Diagnostics.  "ws_profile": after pinb200_set_option("ws_profile", 1), every wsq_decode_kernel launch records per-warp
-   cycle counters; this copies them to `host_out` as uint64 [148 CTAs][20 warps][8 phases] (count = elements). */
+   cycle counters; this copies them to `host_out` as uint64 [132 CTAs][16 warps][8 phases] (count = elements). */
 int pinb200_debug_read(const char* what, void* host_out, int64_t count);
 
 /* Outputs of the fused query; any pointer may be NULL to skip that output. */

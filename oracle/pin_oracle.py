@@ -1,7 +1,7 @@
 """CPU oracle for the PIN-SLAM hot path  --  TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 
 This file restates, op by op in plain PyTorch (CPU by default), the algorithm
-of the reference's per-frame data-parallel hot path so that the sm_100a CUDA
+of the reference's per-frame data-parallel hot path so that the sm_90a CUDA
 kernels in ``pin_slam_b200/csrc`` can be checked against it.  Only ``tests/``,
 ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline`` / ``--impl
 reference`` legs may import it.  The product path (``pin_slam_b200``) never

@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# Build libpinb200.so (sm_100a) in-tree: every .cu is compiled to build/<name>.o when it (or any header) is newer,
+# Build libpinb200.so (sm_90a, H100) in-tree: every .cu is compiled to build/<name>.o when it (or any header) is newer,
 # then linked.  Usage: build.sh [extra nvcc flags]   (extra flags force a full rebuild)
 set -euo pipefail
 here="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
@@ -14,7 +14,7 @@ pids=()
 for src in "$here"/*.cu; do
   o="$obj/$(basename "${src%.cu}").o"
   if [ ! -f "$o" ] || [ "$src" -nt "$o" ] || [ "$newest_hdr" -nt "$o" ]; then
-    ( nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xptxas -v "$@" \
+    ( nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xptxas -v "$@" \
            -c -o "$o" "$src" > "$o.log" 2>&1 || { cat "$o.log"; rm -f "$o"; exit 1; } ) &
     pids+=($!)
   fi
@@ -23,6 +23,6 @@ fail=0
 for p in "${pids[@]:-}"; do [ -n "$p" ] && { wait "$p" || fail=1; }; done
 cat "$obj"/*.o.log >> "$log" 2>/dev/null || true
 [ $fail -eq 0 ] || { grep -E "error" "$log" | head -40; exit 1; }
-nvcc -gencode arch=compute_100a,code=sm_100a -shared -Xcompiler -fPIC -o "$out" "$obj"/*.o
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -Xcompiler -fPIC -o "$out" "$obj"/*.o
 grep -E "error|warning: v|spill|Used" "$log" | grep -vE "^$" | tail -${PINB_BUILD_TAIL:-12} || true
 echo "built $out"

@@ -31,7 +31,7 @@ int sm_count() {
   if (dev != cached_dev) {
     cudaDeviceGetAttribute(&cached, cudaDevAttrMultiProcessorCount, dev);
     cached_dev = dev;
-    if (cached <= 0) cached = 148;
+    if (cached <= 0) cached = 132;
   }
   return cached;
 }

@@ -1,19 +1,17 @@
-// K1b on the 5th-generation tensor cores: the decode launch of the split pipeline for weighted_first maps.
+// K1b on the Hopper warpgroup tensor cores: the phase-synchronous decode launch of the split pipeline for
+// weighted_first maps (decode_variant 0; wsq.cu is the warp-specialised default).
 //
-// One CTA of 128 threads per SM works on tiles of 128 queries (thread t <-> row t <-> TMEM lane t; warp w owns the
-// stash blocks of queries 32w..32w+31 of the tile).  The decoder is a chain of [128 x K] x [K x 64] contractions:
-// every layer is issued by ONE thread as tcgen05.mma (kind::tf32, M = 128, cta_group::1) instructions that read both
-// operands from shared memory in the no-swizzle canonical K-major layout (8-row x 16-byte core matrices) and
-// accumulate in TMEM; the 3xTF32 split (a_hi b_hi + a_lo b_hi + a_hi b_lo, see mlp_mma.cuh) becomes three MMAs per
-// 8-wide k-step.  Completion is signalled through tcgen05.commit -> mbarrier; the epilogue of a layer is
-// tcgen05.ld (32 lanes x 64 columns per warp) -> bias / ReLU / mask in registers -> hi/lo split -> the next layer's
-// A operand, written straight into the canonical layout with 16-byte stores (a thread owns a row, a quarter warp
-// writes one 128-byte core matrix: conflict free).  The backward pass to the decoder input uses transposed copies
-// of the weights staged once per CTA (tf32 MN-major operands need a swizzled layout that cannot double as the
-// K-major forward copy; measured with scripts/micro/umma_test.cu).
-//
-// Compared with the warp-level mma.sync decoder (query_kernel): ~40 tcgen05.mma per 128 rows instead of ~2500 HMMA
-// per 128 rows, 4x the tensor throughput per SM (2048 vs 512 TF32 MAC/clk), no 128-register accumulators.
+// One CTA of 512 threads per SM works on tiles of 128 queries (warp w = row quadrant rq = w & 3, column block
+// cb = w >> 2; thread <-> row 32 rq + lane of the tile; warp w owns the stash blocks of queries 32 rq .. 32 rq + 31).
+// The decoder is a chain of [128 x K] x [K x 64] contractions: every layer is issued by the four warpgroups as
+// wgmma.mma_async (kind tf32, M = 64, twice per tile) reading both operands from shared memory in the no-swizzle
+// canonical K-major layout (8-row x 16-byte core matrices); warpgroup cb computes the 16 accumulator columns of its
+// column block, so a thread's row/column block is produced inside its own warpgroup.  The 3xTF32 split
+// (a_hi b_hi + a_lo b_hi + a_hi b_lo, see mlp_mma.cuh) becomes three MMAs per 8-wide k-step.  The accumulator
+// fragments are handed to the row owners through the consumed A tile; the epilogue then applies bias / ReLU / mask in
+// registers -> hi/lo split -> the next layer's A operand, written straight into the canonical layout with 16-byte
+// stores.  The backward pass to the decoder input uses transposed copies of the weights staged once per CTA (tf32
+// wgmma operands must be K-major).
 #pragma once
 
 #include "umma_common.cuh"
@@ -27,18 +25,71 @@ struct UmmaLayout {  // byte offsets from the 1024-byte aligned dynamic shared m
   int b0, b1, wout, bout;              // fp32 vectors
   int warp0, warp_stride;              // per row-quadrant blocks: Stash | a[8][32]
   int part;                            // [4][4][128] partial output-head sums per column block
-  int bar, tmem;                       // mbarrier (8 B), TMEM base address (4 B)
   int total;
 };
 
-// The CTA: 16 warps on ONE 128-row tile at a time.  Warp w = (row quadrant rq = w & 3, column block cb = w >> 2):
-// TMEM lanes 32 rq .. 32 rq + 31 are the only ones a warp may read, so the four warps of a quadrant split the 64
-// accumulator columns 16 each; the gather phases (A2 / C1) give every warp 8 of the 128 queries.  Four resident
-// warps per scheduler hide the ALU / shared-memory / L2 latencies that a single 4-warp group per SM could not
-// (profiles/r02_k1b_umma_v1: 6.1 cycles per issued instruction with one warp per scheduler).
+// The CTA: 16 warps on ONE 128-row tile at a time.  Warp w = (row quadrant rq = w & 3, column block cb = w >> 2): the
+// four warps of a quadrant split the 64 accumulator columns 16 each; the gather phases (A2 / C1) give every warp 8 of
+// the 128 queries.  Four resident warps per scheduler hide the ALU / shared-memory / L2 latencies.
 constexpr int UM_THREADS = 512;
-constexpr int UM_CB = 4;        // column blocks
+constexpr int UM_CB = 4;        // column blocks (= warpgroups)
 constexpr int UM_CW = 16;       // columns per block
+
+// D[128 x 16] = A[128 x 8 ksteps] B^T (3xTF32) for the columns 16 cb .. 16 cb + 15 (rows of B) that warpgroup cb owns,
+// skipped where 16 cb >= N.  The fragments pass through `xch` (the consumed a_lo tile) so that thread `row` of the
+// warpgroup receives its row's 16 columns in v.  Starts after um_publish_and_sync(); ends with a block barrier, after
+// which the A tiles may be rewritten.
+__device__ __forceinline__ void um_gemm_rows(uint32_t a_hi, uint32_t a_lo, uint32_t a_sbo, uint32_t b_hi, uint32_t b_lo,
+                                             uint32_t b_sbo, int ksteps, int N, int cb, float* xch, int row,
+                                             uint32_t (&v)[UM_CW]) {
+  const bool active = cb * UM_CW < N;
+  const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+  float acc[2][8];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[h][e] = 0.f;
+  if (active) {
+    const uint32_t bh = b_hi + 2 * cb * b_sbo, bl = b_lo + 2 * cb * b_sbo;  // two 8-row groups of B per column block
+    wg_fence();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t ah = a_hi + h * 8 * a_sbo, al = a_lo + h * 8 * a_sbo;
+      for (int s = 0; s < ksteps; ++s) {
+        const uint64_t dah = um_desc(ah + s * 2 * UM_A_LBO, UM_A_LBO, a_sbo), dal = um_desc(al + s * 2 * UM_A_LBO, UM_A_LBO, a_sbo);
+        const uint64_t dbh = um_desc(bh + s * 2 * UM_W_LBO, UM_W_LBO, b_sbo), dbl = um_desc(bl + s * 2 * UM_W_LBO, UM_W_LBO, b_sbo);
+        wg_mma_n16(acc[h], dal, dbh, s > 0);  // small terms first
+        wg_mma_n16(acc[h], dah, dbl, 1);
+        wg_mma_n16(acc[h], dah, dbh, 1);
+      }
+    }
+    wg_commit();
+    wg_wait0();
+  }
+  __syncthreads();  // every warpgroup's MMAs have read the A tiles: a_lo becomes the exchange buffer
+  float* x = xch + cb * (UM_ROWS * UM_CW);
+  if (active) {
+    const int g = lane >> 2, c = lane & 3;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int r0 = 64 * h + 16 * wq + g;
+        *reinterpret_cast<float2*>(x + r0 * UM_CW + 8 * j + 2 * c) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
+        *reinterpret_cast<float2*>(x + (r0 + 8) * UM_CW + 8 * j + 2 * c) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+      }
+  }
+  asm volatile("bar.sync %0, 128;" ::"r"(1 + cb) : "memory");  // the warpgroup's exchange block is complete
+#pragma unroll
+  for (int e4 = 0; e4 < UM_CW / 4; ++e4) {
+    const float4 t = active ? *reinterpret_cast<const float4*>(x + row * UM_CW + 4 * e4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    v[4 * e4] = __float_as_uint(t.x);
+    v[4 * e4 + 1] = __float_as_uint(t.y);
+    v[4 * e4 + 2] = __float_as_uint(t.z);
+    v[4 * e4 + 3] = __float_as_uint(t.w);
+  }
+  __syncthreads();  // the exchange buffer is read before the A tiles are rewritten
+}
 
 template <int FT>
 __global__ void __launch_bounds__(UM_THREADS, 1) decode_umma_kernel(const __grid_constant__ QueryParams p, const UmmaLayout lay) {
@@ -53,7 +104,7 @@ __global__ void __launch_bounds__(UM_THREADS, 1) decode_umma_kernel(const __grid
   unsigned char* sm = um_smem;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int rq = warp & 3, cb = warp >> 2;
-  const int row = rq * WT + lane;  // row of the 128-row tile == TMEM lane
+  const int row = rq * WT + lane;  // row of the 128-row tile
   const pinb200_map_view& m = p.map;
   const int K = p.opts.nn_k, L = p.dec.n_hidden, OC = p.dec.out_dim;
   const bool need_grad = p.opts.need_grad != 0, leaky = p.dec.leaky_relu != 0;
@@ -78,18 +129,9 @@ __global__ void __launch_bounds__(UM_THREADS, 1) decode_umma_kernel(const __grid
   unsigned char* a_hi = sm + lay.a_hi;
   unsigned char* a_lo = sm + lay.a_lo;
   float* s_g = reinterpret_cast<float*>(sm + lay.a_hi);  // row-major [128][GLD] input gradient (aliases the A tile)
-  const uint32_t bar = um_smem_u32(sm + lay.bar);
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(sm + lay.tmem);
+  float* xch = reinterpret_cast<float*>(sm + lay.a_lo);  // accumulator exchange (see um_gemm_rows)
 
-  // ---- one-off: TMEM, mbarrier, weights
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(um_smem_u32(s_tmem)), "r"(64));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(1));
-    asm volatile("fence.mbarrier_init.release.cluster;");
-  }
+  // ---- one-off: weights
   um_stage_weight(p.dec.w[0], D, H, D, H, K0, false, sm + lay.w0f_hi, sm + lay.w0f_lo);
   if (need_grad) um_stage_weight(p.dec.w[0], D, D, H, N0, H, true, sm + lay.w0b_hi, sm + lay.w0b_lo);
   if (L > 1) {
@@ -103,9 +145,6 @@ __global__ void __launch_bounds__(UM_THREADS, 1) decode_umma_kernel(const __grid
   for (int e = tid; e < OC * H; e += UM_THREADS) reinterpret_cast<float*>(sm + lay.wout)[e] = __ldg(p.dec.w_out + e);
   if (tid < 4) reinterpret_cast<float*>(sm + lay.bout)[tid] = (p.dec.b_out && tid < OC) ? __ldg(p.dec.b_out + tid) : 0.f;
   um_publish_and_sync();
-  const uint32_t tmem_d = *s_tmem;
-  const uint32_t taddr = tmem_d + ((uint32_t)(rq * 32) << 16) + (uint32_t)(cb * UM_CW);  // lanes of rq, columns of cb
-  uint32_t phase = 0;
 
   const uint32_t a_hi_u = um_smem_u32(a_hi), a_lo_u = um_smem_u32(a_lo);
   const uint32_t w0f_hi = um_smem_u32(sm + lay.w0f_hi), w0f_lo = um_smem_u32(sm + lay.w0f_lo);
@@ -197,13 +236,11 @@ __global__ void __launch_bounds__(UM_THREADS, 1) decode_umma_kernel(const __grid
       }
     }
 
-    // ============ B: decoder forward on tcgen05 ============
+    // ============ B: decoder forward on wgmma ============
     uint32_t v[UM_CW];
     uint32_t mk0 = 0u, mkL = 0u;  // ReLU masks (this thread's 16 columns) of layer 0 and of the last hidden layer
     um_publish_and_sync();
-    if (tid == 0) um_issue_gemm(tmem_d, a_hi_u, a_lo_u, A_SBO0, w0f_hi, w0f_lo, W_SBO0, K0 / 8, H, bar);
-    um_wait(bar, phase);
-    um_tmem_ld16(taddr, v);
+    um_gemm_rows(a_hi_u, a_lo_u, A_SBO0, w0f_hi, w0f_lo, W_SBO0, K0 / 8, H, cb, xch, row, v);
     if (L > 1) {
       // layer-0 epilogue: bias, ReLU (mask kept), split, next A operand
 #pragma unroll
@@ -225,9 +262,7 @@ __global__ void __launch_bounds__(UM_THREADS, 1) decode_umma_kernel(const __grid
         *reinterpret_cast<float4*>(a_lo + off) = lo;
       }
       um_publish_and_sync();
-      if (tid == 0) um_issue_gemm(tmem_d, a_hi_u, a_lo_u, A_SBO1, w1f_hi, w1f_lo, W_SBO1, H / 8, H, bar);
-      um_wait(bar, phase);
-      um_tmem_ld16(taddr, v);
+      um_gemm_rows(a_hi_u, a_lo_u, A_SBO1, w1f_hi, w1f_lo, W_SBO1, H / 8, H, cb, xch, row, v);
     }
     // last hidden layer: bias, ReLU (mask kept), this column block's part of the output head(s)
     {
@@ -280,9 +315,7 @@ __global__ void __launch_bounds__(UM_THREADS, 1) decode_umma_kernel(const __grid
         }
         if (L > 1) {
           um_publish_and_sync();
-          if (tid == 0) um_issue_gemm(tmem_d, a_hi_u, a_lo_u, A_SBO1, w1b_hi, w1b_lo, W_SBO1, H / 8, H, bar);
-          um_wait(bar, phase);
-          um_tmem_ld16(taddr, v);
+          um_gemm_rows(a_hi_u, a_lo_u, A_SBO1, w1b_hi, w1b_lo, W_SBO1, H / 8, H, cb, xch, row, v);
 #pragma unroll
           for (int cc = 0; cc < UM_CW / 4; ++cc) {
             float g[4] = {__uint_as_float(v[4 * cc]), __uint_as_float(v[4 * cc + 1]), __uint_as_float(v[4 * cc + 2]),
@@ -298,11 +331,11 @@ __global__ void __launch_bounds__(UM_THREADS, 1) decode_umma_kernel(const __grid
           }
         }
         um_publish_and_sync();
-        if (tid == 0) um_issue_gemm(tmem_d, a_hi_u, a_lo_u, A_SBO1, w0b_hi, w0b_lo, W_SBO1, H / 8, N0, bar);
+        um_gemm_rows(a_hi_u, a_lo_u, A_SBO1, w0b_hi, w0b_lo, W_SBO1, H / 8, N0, cb, xch, row, v);
       } else {
         __syncthreads();  // output-head partial sums of the other column blocks
       }
-      // decoder outputs of this row (the barrier above ordered the partial sums)
+      // decoder outputs of this row (the barriers above ordered the partial sums)
       if (c == 0) {
 #pragma unroll
         for (int ch = 0; ch < 4; ++ch)
@@ -322,8 +355,6 @@ __global__ void __launch_bounds__(UM_THREADS, 1) decode_umma_kernel(const __grid
       const float val_c = c == 0 ? val[0] : (c == 1 ? val[1] : (c == 2 ? val[2] : val[3]));
       const float dv_c = c == 0 ? dvv[0] : (c == 1 ? dvv[1] : (c == 2 ? dvv[2] : dvv[3]));
       if (need_grad) {
-        um_wait(bar, phase);
-        um_tmem_ld16(taddr, v);
         // every row of the A tile has been consumed by the MMA: the tile becomes the row-major input gradient
         if (cb * UM_CW < K0) {
 #pragma unroll
@@ -445,11 +476,6 @@ __global__ void __launch_bounds__(UM_THREADS, 1) decode_umma_kernel(const __grid
       if (need_grad && c + 1 < n_pass) __syncthreads();
     }
   }
-
-  // ---- teardown
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(64));
 }
 
 // ---------------------------------------------------------------------------
@@ -482,6 +508,7 @@ static UmmaLayout plan_umma_layout(const pinb200_decoder_view& d, bool need_grad
   }
   const int a_bytes = (UM_ROWS / 8) * (64 / 4) * UM_A_LBO;  // K = 64
   static_assert(UM_ROWS * UmmaDims<FT>::GLD * 4 <= (UM_ROWS / 8) * (64 / 4) * UM_A_LBO, "gradient tile must fit the A tile");
+  static_assert(UM_CB * UM_ROWS * UM_CW * 4 <= (UM_ROWS / 8) * (64 / 4) * UM_A_LBO, "accumulator exchange must fit the A tile");
   l.a_hi = take(a_bytes);
   l.a_lo = take(a_bytes);
   l.b0 = take(64 * 4);
@@ -491,8 +518,6 @@ static UmmaLayout plan_umma_layout(const pinb200_decoder_view& d, bool need_grad
   l.warp_stride = (Stash::floats + WT * 8) * 4;
   l.warp0 = take(4 * l.warp_stride);
   l.part = take(4 * 4 * UM_ROWS * 4);
-  l.bar = take(8);
-  l.tmem = take(4);
   l.total = o;
   return l;
 }
@@ -529,7 +554,7 @@ static int launch_decode_umma(QueryParams& p, cudaStream_t stream) {
   return check_launch("decode_umma_kernel");
 }
 
-// the tcgen05 decode covers weighted_first maps with a 1- or 2-layer 64-wide decoder and F in {8, 16, 32}
+// the tensor-core decode covers weighted_first maps with a 1- or 2-layer 64-wide decoder and F in {8, 16, 32}
 static bool umma_decode_supported(const QueryParams& p) {
   const int F = p.dec.in_dim - 3;
   return p.opts.weighted_first && p.dec.hidden_dim == 64 && p.dec.n_hidden >= 1 && p.dec.n_hidden <= 2 &&

@@ -78,15 +78,10 @@ __device__ __forceinline__ void stage_decoder(const pinb200_decoder_view& d, con
   for (int e = tid; e < align4(d.out_dim); e += nt) bo[e] = (d.b_out && e < d.out_dim) ? __ldg(d.b_out + e) : 0.f;
 }
 
-// Packed fp32 FMA (Blackwell FFMA2): {d0,d1} += {a0,a1} * b.  One issue slot for two FMAs; ptxas folds the
-// broadcast operand into FFMA2's scalar .F32 source, so a 128-bit weight load feeds exactly two instructions.
+// {d0,d1} += {a0,a1} * b, two round-to-nearest fp32 FMAs (Hopper has no packed fp32 FMA)
 __device__ __forceinline__ void ffma2(float& d0, float& d1, float a0, float a1, float b) {
-  unsigned long long d, a, bb;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(a) : "f"(a0), "f"(a1));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(bb) : "f"(b), "f"(b));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "f"(d0), "f"(d1));
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(d) : "l"(a), "l"(bb));
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d0), "=f"(d1) : "l"(d));
+  d0 = fmaf(a0, b, d0);
+  d1 = fmaf(a1, b, d1);
 }
 
 // out[o] = bias[o] + sum_i w[i][o] * col[i*ACT_LD]   (w: [n_in][NOUT] in smem, warp-uniform float4 reads)

@@ -12,7 +12,7 @@
 // two B values of a lane become adjacent in the nn.Linear row: one LDS.64 per (hi | lo) fragment instead of two
 // LDS.32.  Leading dimensions == 8 (mod 32) make those 64-bit fragment loads bank-conflict free.
 //
-// (tcgen05/TMEM needs M >= 64 rows and a block-wide TMEM/mbarrier choreography; with independent 32-row warp
+// (wgmma needs 64-row warpgroup tiles and a warpgroup-wide issue / wait choreography; with independent 32-row warp
 // tiles the warp-synchronous mma.sync form is the natural fit.  DESIGN.md section 7 discusses the trade-off.)
 #pragma once
 #include "mlp_mma.cuh"

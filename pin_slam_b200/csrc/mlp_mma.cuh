@@ -10,7 +10,7 @@
 // (row = lane/4, col = lane%4) is bank-conflict free); weights in the torch nn.Linear layout [out][in] with
 // leading dimension in_pad + 4 for the same reason.
 //
-// (tcgen05/TMEM needs M >= 64 rows and a block-wide TMEM/mbarrier choreography; with independent 32-row warp
+// (wgmma needs 64-row warpgroup tiles and a warpgroup-wide issue / wait choreography; with independent 32-row warp
 // tiles the warp-synchronous mma.sync form is the natural fit.  DESIGN.md section 7 discusses the trade-off.)
 #pragma once
 #include "common.cuh"

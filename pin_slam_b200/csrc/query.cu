@@ -31,7 +31,7 @@ template <bool SEEDS>
 __global__ void __launch_bounds__(128, 4) search_kernel(const __grid_constant__ QueryParams p) {
   extern __shared__ __align__(16) float smem[];
   uint32_t* s_delta = reinterpret_cast<uint32_t*>(smem);
-  // programmatic dependent launch: the decode launch may start its prologue (TMEM, mbarriers, weight staging) on the
+  // programmatic dependent launch: the decode launch may start its prologue (mbarriers, weight staging) on the
   // SMs this grid's tail frees; it waits (griddepcontrol.wait) before it reads anything written here
   asm volatile("griddepcontrol.launch_dependents;");
   fill_probe_deltas(p.map, s_delta);
@@ -710,7 +710,7 @@ extern "C" int pinb200_query_sdf(const pinb200_map_view* map, const pinb200_deco
   // Large batches run as two launches (search at high occupancy, then decode) through the caller's workspace; small
   // ones (tracker / mapper sized, latency-bound) stay fused in one launch.
   const int64_t need = pinb200_query_workspace_bytes(n);
-  // weighted_first maps with a tcgen05-decodable configuration: the two-launch pipeline wins from ~1 k queries on
+  // weighted_first maps with a wgmma-decodable configuration: the two-launch pipeline wins from ~1 k queries on
   // (8 k queries, F = 32: 48 us vs 72 us for the fused launch; scripts/exp_small_n.py)
   QueryParams probe{};
   probe.dec = *sdf_dec;
@@ -727,7 +727,7 @@ extern "C" int pinb200_query_sdf(const pinb200_map_view* map, const pinb200_deco
     rc = launch_search(p, (cudaStream_t)stream);
     if (rc) return rc;
   }
-  // decode: tcgen05 tiles of 128 queries where the configuration allows it, else the warp-level mma.sync kernel
+  // decode: wgmma tiles of 128 queries where the configuration allows it, else the warp-level mma.sync kernel
   p.pdl = split ? 1 : 0;  // only the launch that directly follows the search launch
   auto decode = [&](QueryParams& qp) {
     if (split && umma_decode_supported(qp))
@@ -769,7 +769,7 @@ extern "C" int pinb200_set_option(const char* name, int64_t value) {
     g_split_min_queries_wf = value > 0 ? value : PINB200_SPLIT_MIN_QUERIES_WF;
   } else if (key == "decode_variant") {
     if (value < 0 || value > 1) {
-      set_error("set_option: decode_variant %lld (0: phase-synchronous tcgen05 decode, 1: warp-specialised)", (long long)value);
+      set_error("set_option: decode_variant %lld (0: phase-synchronous wgmma decode, 1: warp-specialised)", (long long)value);
       return PINB200_ERR_BAD_ARG;
     }
     g_decode_variant = (int)value;

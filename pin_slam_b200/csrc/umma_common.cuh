@@ -1,5 +1,10 @@
-// tcgen05 / TMEM building blocks shared by the tensor-core decode kernels (decode_umma.cuh, wsq.cu): shared-memory
-// matrix descriptors of the no-swizzle canonical K-major layout, MMA issue, mbarrier wait, TMEM loads, TF32 hi/lo split.
+// Hopper warpgroup-MMA (wgmma) building blocks shared by the tensor-core decode kernels (decode_umma.cuh, wsq.cu):
+// shared-memory matrix descriptors of the no-swizzle canonical K-major layout, wgmma issue (operands from shared memory
+// or, for A, from registers), TF32 hi/lo split, weight staging.
+//
+// Accumulator fragment of a 64 x N wgmma (per warpgroup of 128 threads): warp w of the group, lane l, g = l / 4,
+// c = l % 4 holds for every 8-column block j: d[4j + 0, 1] = rows 16w + g, columns 8j + 2c, 8j + 2c + 1 and
+// d[4j + 2, 3] = row 16w + g + 8, same columns.
 #pragma once
 #include "mlp_mma.cuh"
 
@@ -13,89 +18,69 @@ constexpr int UM_W_LBO = 128;
 
 __device__ __forceinline__ uint32_t um_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
+// wgmma matrix descriptor, no swizzle: LBO = bytes between core matrices along K, SBO = bytes between 8-row groups
 __device__ __forceinline__ uint64_t um_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
-  d |= 1ull << 46;  // descriptor version (sm_100)
-  return d;         // base offset 0, layout type 0 = no swizzle
+  return d;  // base offset 0, layout type 0 = no swizzle
 }
-// instruction descriptor: D fp32, A/B tf32, both K-major, dense
-__device__ __forceinline__ uint32_t um_idesc(int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(UM_ROWS >> 4) << 24);
-}
-__device__ __forceinline__ void um_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
+
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D[64 x 16] (+)= A B^T, tf32, both operands from shared memory
+__device__ __forceinline__ void wg_mma_n16(float (&d)[8], uint64_t adesc, uint64_t bdesc, int acc) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(acc)
       : "memory");
 }
-// D[128 x N] = A[128 x 8*ksteps] B^T with the 3xTF32 split; issued by one thread, completion arrives on `bar`
-__device__ __forceinline__ void um_issue_gemm(uint32_t tmem_d, uint32_t a_hi, uint32_t a_lo, uint32_t a_sbo, uint32_t b_hi,
-                                              uint32_t b_lo, uint32_t b_sbo, int ksteps, int N, uint32_t bar) {
-  const uint32_t idesc = um_idesc(N);
-  for (int s = 0; s < ksteps; ++s) {
-    const uint64_t ah = um_desc(a_hi + s * 2 * UM_A_LBO, UM_A_LBO, a_sbo);
-    const uint64_t al = um_desc(a_lo + s * 2 * UM_A_LBO, UM_A_LBO, a_sbo);
-    const uint64_t bh = um_desc(b_hi + s * 2 * UM_W_LBO, UM_W_LBO, b_sbo);
-    const uint64_t bl = um_desc(b_lo + s * 2 * UM_W_LBO, UM_W_LBO, b_sbo);
-    um_mma(tmem_d, al, bh, idesc, s > 0);  // small terms first
-    um_mma(tmem_d, ah, bl, idesc, 1);
-    um_mma(tmem_d, ah, bh, idesc, 1);
-  }
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 
-__device__ __forceinline__ void um_wait(uint32_t bar, uint32_t& phase) {
-  // one lane per warp polls (try_wait suspends in hardware for a while; 512 pollers would burn the issue slots the
-  // other warps need), the rest of the warp joins at the __syncwarp.  Bounded: a mis-programmed MMA must trap, not hang.
-  if ((threadIdx.x & 31) == 0) {
-    uint32_t done = 0;
-    for (int it = 0; it < (1 << 24) && !done; ++it) {
-      asm volatile(
-          "{\n\t.reg .pred P1;\n\t"
-          "mbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2;\n\t"
-          "selp.b32 %0, 1, 0, P1;\n\t}\n"
-          : "=r"(done)
-          : "r"(bar), "r"(phase)
-          : "memory");
-    }
-    if (!done) __trap();
-  }
-  __syncwarp();
-  phase ^= 1u;
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
+#define PINB_WG_D32                                                                                                  \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, " \
+  "%24, %25, %26, %27, %28, %29, %30, %31}"
+#define PINB_WG_D32_OPS                                                                                                \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),         \
+      "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),          \
+      "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),         \
+      "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
 
-__device__ __forceinline__ void um_tmem_ld64(uint32_t taddr, uint32_t (&v)[64]) {
+// D[64 x 64] (+)= A B^T, tf32, both operands from shared memory
+__device__ __forceinline__ void wg_mma_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, int acc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x64.b32"
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, "
-      "%25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, [%64];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31]), "=r"(v[32]),
-        "=r"(v[33]), "=r"(v[34]), "=r"(v[35]), "=r"(v[36]), "=r"(v[37]), "=r"(v[38]), "=r"(v[39]), "=r"(v[40]),
-        "=r"(v[41]), "=r"(v[42]), "=r"(v[43]), "=r"(v[44]), "=r"(v[45]), "=r"(v[46]), "=r"(v[47]), "=r"(v[48]),
-        "=r"(v[49]), "=r"(v[50]), "=r"(v[51]), "=r"(v[52]), "=r"(v[53]), "=r"(v[54]), "=r"(v[55]), "=r"(v[56]),
-        "=r"(v[57]), "=r"(v[58]), "=r"(v[59]), "=r"(v[60]), "=r"(v[61]), "=r"(v[62]), "=r"(v[63])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " PINB_WG_D32 ", %32, %33, p, 1, 1;\n\t}\n"
+      : PINB_WG_D32_OPS
+      : "l"(adesc), "l"(bdesc), "r"(acc)
+      : "memory");
 }
+
+// D[64 x 64] (+)= A B^T, tf32, A (64 x 8) from registers in the m16n8k8 A-fragment order
+// (a0: row g, k c; a1: row g + 8, k c; a2: row g, k c + 4; a3: row g + 8, k c + 4), B from shared memory
+__device__ __forceinline__ void wg_mma_n64_rs(float (&d)[32], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
+                                              uint64_t bdesc, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " PINB_WG_D32 ", {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}\n"
+      : PINB_WG_D32_OPS
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(acc)
+      : "memory");
+}
+#undef PINB_WG_D32
+#undef PINB_WG_D32_OPS
 
 // make the generic-proxy shared-memory writes of every thread visible to the tensor core, then meet
 __device__ __forceinline__ void um_publish_and_sync() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
 __device__ __forceinline__ void um_split4(const float4 v, float4& hi, float4& lo) {
@@ -112,16 +97,23 @@ __device__ __forceinline__ void um_split4(const float4 v, float4& hi, float4& lo
 // byte offset of the 16-byte chunk (row m, columns 4*c .. 4*c+3) of an A tile with K columns
 __device__ __forceinline__ int um_a_off(int m, int c, int K) { return (m >> 3) * ((K >> 2) * UM_A_LBO) + c * UM_A_LBO + (m & 7) * 16; }
 
+// position of column c inside its 8-column k-step when the A operand comes from accumulator registers: register
+// fragment slot k (0..3) carries accumulator column 2k, slot k + 4 column 2k + 1 (see wg_mma_n64_rs)
+__device__ __forceinline__ int um_kperm(int c) { return (c & ~7) | ((c & 1) ? 4 + ((c & 7) >> 1) : ((c & 7) >> 1)); }
+
 // stage the canonical K-major B tile of `rows` x `cols`: element (r, c) = src[r][c] (or src[c][r] when `transpose`) for
-// r < rows_src, c < cols_src, zero elsewhere; `src_ld` = leading dimension of the row-major source
+// r < rows_src, c < cols_src, zero elsewhere; `src_ld` = leading dimension of the row-major source.  `kperm` stores
+// column c at um_kperm(c), for an A operand taken from accumulator registers.
 __device__ __forceinline__ void um_stage_weight(const float* __restrict__ src, int src_ld, int rows_src, int cols_src, int rows,
-                                                int cols, bool transpose, unsigned char* hi, unsigned char* lo) {
+                                                int cols, bool transpose, unsigned char* hi, unsigned char* lo,
+                                                bool kperm = false) {
   for (int e = threadIdx.x; e < rows * cols; e += blockDim.x) {
     const int r = e / cols, c = e - r * cols;
     float w = 0.f;
     if (r < rows_src && c < cols_src) w = transpose ? __ldg(src + (size_t)c * src_ld + r) : __ldg(src + (size_t)r * src_ld + c);
     const float h = __uint_as_float(__float_as_uint(w) & TF32_MASK);
-    const int off = (r >> 3) * ((cols >> 2) * UM_W_LBO) + (c >> 2) * UM_W_LBO + (r & 7) * 16 + (c & 3) * 4;
+    const int cs = kperm ? um_kperm(c) : c;
+    const int off = (r >> 3) * ((cols >> 2) * UM_W_LBO) + (cs >> 2) * UM_W_LBO + (r & 7) * 16 + (cs & 3) * 4;
     *reinterpret_cast<float*>(hi + off) = h;
     *reinterpret_cast<float*>(lo + off) = w - h;
   }
@@ -130,19 +122,8 @@ __device__ __forceinline__ void um_stage_weight(const float* __restrict__ src, i
 template <int FT>
 struct UmmaDims {
   static constexpr int K0 = (FT + 3 + 7) / 8 * 8;  // decoder input width padded to the MMA k-step
-  static constexpr int N0 = (K0 + 15) / 16 * 16;   // N of the input-gradient MMA (multiple of 16 for M = 128)
+  static constexpr int N0 = (K0 + 15) / 16 * 16;   // N of the input-gradient MMA (whole 16-column blocks)
   static constexpr int GLD = K0 + 4;               // leading dimension (floats) of the row-major input-gradient tile
 };
-
-// 16-column TMEM load: lane t of the warp reads columns [col, col+16) of TMEM lane (lane quadrant base + t)
-__device__ __forceinline__ void um_tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32"
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 
 }  // namespace pinb

@@ -8,21 +8,19 @@
 //   G  gather teams   (2 x 4 warps, 120 registers) F/4 lanes per feature row (a 128-byte row = 8 lanes x LDG.128): ONE pass
 //                     over the K rows gives the IDW-interpolated feature  xbar = sum_k w_k f_k  AND its three directional
 //                     derivatives  T_j = sum_k omega_kj (f_k - f_0)  -> rows of an A tile (canonical K-major, hi / lo TF32)
-//   M  MMA warps      (one per epilogue group, the elected lane issues) layer 0 as tcgen05.mma with the A tile from shared
-//                     memory, layer 1 with the A operand IN TENSOR MEMORY, chunk by chunk behind the layer-0 epilogue;
-//                     layer 0 of the next tile right behind layer 1 of this one (separate accumulator columns)
-//   E  epilogue groups (2 x 4 warps, one TMEM lane quadrant per warp): thread = tile row.  tcgen05.ld of the accumulator,
-//                     ReLU gate, hi / lo split, tcgen05.st of the next layer's A operand back to TMEM, mbarrier arrive;
-//                     last layer: output head in registers, results to global memory.  Never issues an MMA, never meets
-//                     another warp at a barrier.
+//   C  consumer       (one warpgroup, 216 registers) layer 0 as wgmma.mma_async with the A tile from shared memory (two
+//                     64-row halves, accumulators in registers), then releases the A tile to its gather team; ReLU gate,
+//                     hi / lo split in registers, layer 1 with the A operand IN REGISTERS (the accumulator fragment is the
+//                     A fragment once the k order inside a k-step is permuted, see um_kperm: the layer-1 weights are staged
+//                     in that order); last layer: output head in registers (quad shuffles), results to global memory.
 //
 // d sdf / d q is computed in FORWARD mode: a tile row is either a value row (decoder input x) or one of the three
 // tangent rows (dx / dq_j) of the same query; tangent rows go through the same weights, without bias, and are gated
-// by the value row's ReLU pattern.  Rows 4i .. 4i+3 of a tile belong to query i, so the gate is a quad shuffle.  This
-// needs no transposed weight copies (52 KB instead of 108 KB of decoder state), no backward MMAs, no second pass over
-// the feature rows (the C1 phase of decode_umma_kernel: 6.4 M sectors per 200 k queries) and no input-gradient tile,
-// which is what makes room for a ring of A tiles: the gathers of later tiles run under the MMA chain of tile t.
-// Without d/dq (mesher, dense RGB-D queries) a tile is 128 value rows.
+// by the value row's ReLU pattern.  Rows 4i .. 4i+3 of a tile belong to query i, so in the accumulator fragment the
+// gate comes from the lane four rows up (one shuffle of a 32-bit mask per 64-row half).  This needs no transposed weight
+// copies, no backward MMAs, no second pass over the feature rows (the C1 phase of decode_umma_kernel) and no
+// input-gradient tile, which is what makes room for a ring of A tiles: the gathers of later tiles run under the MMA
+// chain of tile t.  Without d/dq (mesher, dense RGB-D queries) a tile is 128 value rows.
 //
 // Replaces model/neural_points.py:598-731 (gathers, IDW, weighted_first), model/decoder.py:61-85,112 and the autograd
 // call of utils/tools.py:247-260 for batches of >= PINB200_SPLIT_MIN_QUERIES_WF queries (inference mode).
@@ -31,19 +29,16 @@
 
 namespace pinb {
 
-constexpr int WS_EG = 2;       // epilogue groups of 4 warps
+constexpr int WS_CW = 4;       // consumer warps (one warpgroup)
 constexpr int WS_GT = 2;       // gather teams of 4 warps: team t fills the A tiles of the CTA's tiles i = t (mod WS_GT)
 constexpr int WS_GW = 4;       // warps per gather team
-constexpr int WS_LW = 2;       // loader warps; the other two warps of their 4-warp group issue the MMAs (one per epilogue group)
-constexpr int WS_THREADS = (4 * WS_EG + WS_GT * WS_GW + WS_LW + WS_EG) * 32;
-static_assert((WS_LW + WS_EG) % 4 == 0, "setmaxnreg works on groups of 4 warps");
+constexpr int WS_LW = 4;       // loader warps
+constexpr int WS_THREADS = (WS_CW + WS_GT * WS_GW + WS_LW) * 32;
 // register budget per thread (setmaxnreg, one value per 4-warp group).  The pool is what the CTA was launched with
-// (640 threads x 96 registers): 8*32*80 + 8*32*120 + 4*32*80 = 61440
-constexpr int WS_REG_E = 80, WS_REG_G = 120, WS_REG_L = 80;
-static_assert((4 * WS_EG * WS_REG_E + WS_GT * WS_GW * WS_REG_G + (WS_LW + WS_EG) * WS_REG_L) * 32 <= WS_THREADS * 96, "setmaxnreg pool");
-constexpr int WS_A0 = 2;       // A-tile ring slots, one per gather team / epilogue group pair: layer 0 of a tile is issued early,
-                               // so its slot is free again while the rest of the chain runs (3 slots measured the same)
-constexpr int WS_TCOLS = 256;  // TMEM columns per epilogue group: [0,64) D0, [64,128) A1 hi, [128,192) A1 lo, [192,256) D1
+// (512 threads x 128 registers)
+constexpr int WS_REG_C = 216, WS_REG_G = 120, WS_REG_L = 56;
+static_assert((WS_CW * WS_REG_C + WS_GT * WS_GW * WS_REG_G + WS_LW * WS_REG_L) * 32 <= WS_THREADS * 128, "setmaxnreg pool");
+constexpr int WS_A0 = 2;       // A-tile ring slots, one per gather team
 
 struct WsMeta {  // float offsets inside a meta block of 32 queries, [field][k][lane]
   static constexpr int li = 0;                   // [8][32] neighbour id | REMAP, -1 invalid
@@ -59,18 +54,19 @@ struct WsLayout {  // byte offsets from the dynamic shared memory base
   int w0_hi, w0_lo, w1_hi, w1_lo, b0, b1, wout, bout;
   int a0, a0_half, a0_stride;  // ring of A tiles: slot s = [a0 + s*stride: hi | + half: lo]
   int meta, meta_stride, n_meta;
-  int bars, tmem, total;
+  int bars, total;
 };
 // mbarrier indices
 constexpr int WS_MB_MAX = 16;
 constexpr int WSB_A0_FULL = 0, WSB_A0_EMPTY = WSB_A0_FULL + WS_A0, WSB_META_FULL = WSB_A0_EMPTY + WS_A0,
-              WSB_META_EMPTY = WSB_META_FULL + WS_MB_MAX, WSB_MMA0 = WSB_META_EMPTY + WS_MB_MAX, WSB_MMA1 = WSB_MMA0 + WS_EG,
-              WSB_A1_READY = WSB_MMA1 + WS_EG, WSB_D1_FREE = WSB_A1_READY + 4 * WS_EG, WSB_COUNT = WSB_D1_FREE + WS_EG;
+              WSB_META_EMPTY = WSB_META_FULL + WS_MB_MAX, WSB_COUNT = WSB_META_EMPTY + WS_MB_MAX;
 
-// Optional cycle accounting (pinb200_set_option("ws_profile", 1)): per warp, clock64 deltas of up to 8 phases,
-// summed over the tiles of the launch; read back with pinb200_debug_read("ws_profile", ...).
+// Optional cycle accounting (pinb200_set_option("ws_profile", 1)): per warp, clock deltas of up to 8 phases,
+// summed over the tiles of the launch, for the first WS_PROF_CTAS CTAs; read back with
+// pinb200_debug_read("ws_profile", ...).
 constexpr int WS_PROF_SLOTS = 8;
-__device__ unsigned long long g_ws_prof[148 * (WS_THREADS / 32) * WS_PROF_SLOTS];
+constexpr int WS_PROF_CTAS = 132;  // one CTA per SM of an H100 SXM
+__device__ unsigned long long g_ws_prof[WS_PROF_CTAS * (WS_THREADS / 32) * WS_PROF_SLOTS];
 static int g_ws_profile = 0;
 
 template <bool PROF>
@@ -93,7 +89,7 @@ struct WsClock {  // PROF = false: no code at all (64-bit counters in the produc
   }
   __device__ __forceinline__ void flush(int warp) {
     if (PROF) {
-      if ((threadIdx.x & 31) == 0 && blockIdx.x < 148) {
+      if ((threadIdx.x & 31) == 0 && blockIdx.x < WS_PROF_CTAS) {
 #pragma unroll
         for (int i = 0; i < WS_PROF_SLOTS; ++i) g_ws_prof[(blockIdx.x * (WS_THREADS / 32) + warp) * WS_PROF_SLOTS + i] = acc[i];
       }
@@ -102,10 +98,8 @@ struct WsClock {  // PROF = false: no code at all (64-bit counters in the produc
 };
 
 // mbarrier wait, executed by every lane of a converged warp (ONE warp instruction per attempt).  The suspend-time hint
-// parks the warp in hardware until the phase completes: a software poll loop (round-2 first version: one lane
-// spinning on try_wait, the rest at __syncwarp) made up 65 % of all executed instructions, stole issue slots and
-// instruction-cache bandwidth from the working warps (profiles/r02_wsq_v1: icc hit rate 59 %, no_instruction 3.5 stalls
-// per issue).  Bounded: a mis-programmed pipeline must trap, not hang the GPU.
+// parks the warp in hardware until the phase completes, instead of a software poll loop that steals issue slots from
+// the working warps.  Bounded: a mis-programmed pipeline must trap, not hang the GPU.
 __device__ __forceinline__ void ws_wait(uint32_t bar, uint32_t parity) {
   uint32_t done = 0;
 #pragma unroll 1
@@ -138,57 +132,6 @@ __device__ __forceinline__ void ws_wait_relaxed(uint32_t bar, uint32_t parity) {
 }
 __device__ __forceinline__ void ws_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void ws_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void ws_group_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
-__device__ __forceinline__ void ws_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void ws_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void ws_mma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void ws_tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n" ::"r"(
-          taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]),
-      "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-
-// TMEM load split into issue and wait, so that shared-memory loads can be put under its latency; the wait takes the
-// destination registers as in/out operands to keep their consumers behind it
-__device__ __forceinline__ void ws_tmem_ld16_issue(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32"
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void ws_tmem_ld_wait(uint32_t (&v)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]), "+r"(v[8]),
-                 "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15])::"memory");
-}
-__device__ __forceinline__ void ws_lds16(const float* src, float (&b)[16]) {
-#pragma unroll
-  for (int e4 = 0; e4 < 4; ++e4) {
-    const float4 t = *reinterpret_cast<const float4*>(src + 4 * e4);
-    b[4 * e4] = t.x;
-    b[4 * e4 + 1] = t.y;
-    b[4 * e4 + 2] = t.z;
-    b[4 * e4 + 3] = t.w;
-  }
 }
 
 static_assert(WsMeta::P - WsMeta::om == Seeds::P - Seeds::om && WsMeta::floats_g - WsMeta::om == Seeds::floats,
@@ -231,37 +174,26 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
   const int K = p.opts.nn_k, L = p.dec.n_hidden, OC = p.dec.out_dim;
   const float slope = p.dec.leaky_relu ? 0.01f : 0.f;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm + lay.bars);
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(sm + lay.tmem);
   float* meta = reinterpret_cast<float*>(sm + lay.meta);
   WsClock<PROF> clk;
 
-  // ---- prologue (the only block-wide barrier): TMEM, mbarriers, decoder weights
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(um_smem_u32(s_tmem)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
+  // ---- prologue (the only block-wide barrier): mbarriers, decoder weights
   if (tid == 0) {
     auto init = [&](int i, int count) {
       asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(um_smem_u32(bars + i)), "r"(count));
     };
     for (int s = 0; s < WS_A0; ++s) {
       init(WSB_A0_FULL + s, WS_GW);
-      init(WSB_A0_EMPTY + s, 1);
+      init(WSB_A0_EMPTY + s, WS_CW);
     }
     for (int s = 0; s < WS_MB_MAX; ++s) {
       init(WSB_META_FULL + s, 1);
       init(WSB_META_EMPTY + s, WS_GW);
     }
-    for (int g = 0; g < WS_EG; ++g) {
-      init(WSB_MMA0 + g, 1);
-      init(WSB_MMA1 + g, 1);
-      for (int c = 0; c < 4; ++c) init(WSB_A1_READY + 4 * g + c, 128);
-      init(WSB_D1_FREE + g, 128);
-    }
     asm volatile("fence.mbarrier_init.release.cluster;");
   }
   um_stage_weight(p.dec.w[0], D, H, D, H, K0, false, sm + lay.w0_hi, sm + lay.w0_lo);
-  if (L > 1) um_stage_weight(p.dec.w[1], H, H, H, H, H, false, sm + lay.w1_hi, sm + lay.w1_lo);
+  if (L > 1) um_stage_weight(p.dec.w[1], H, H, H, H, H, false, sm + lay.w1_hi, sm + lay.w1_lo, true);
   __syncthreads();
   // the layer-0 bias rides on the MMA: input column D is 1 for value rows (0 for tangent rows), weight column D = b0
   static_assert(D < K0, "a spare (padding) input column carries the bias");
@@ -279,60 +211,70 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
   for (int e = tid; e < 4 * H; e += WS_THREADS) reinterpret_cast<float*>(sm + lay.wout)[e] = e < OC * H ? __ldg(p.dec.w_out + e) : 0.f;
   if (tid < 4) reinterpret_cast<float*>(sm + lay.bout)[tid] = (p.dec.b_out && tid < OC) ? __ldg(p.dec.b_out + tid) : 0.f;
   um_publish_and_sync();
-  const uint32_t tmem_base = *s_tmem;
   clk.start();
 
   const long long n_tiles = (p.n + QT - 1) / QT;
   const int n_blocks = p.n_tiles;  // 32-query stash blocks
 
-  if (warp < 4 * WS_EG) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(WS_REG_E));
+  if (warp < WS_CW) {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(WS_REG_C));
     // =====================================================================================================
-    // E: epilogue group g owns the tiles i = g, g + 2, ... of this CTA.  Its threads never issue an MMA and never
-    // meet at a barrier: they wait for the group's MMA warp through mbarriers (bar0 / bar1: layer 0 / 1 complete)
-    // and tell it through two more (a1_ready: A1 written + D0 read, d1_free: last accumulator read).
-    // profile slots: 0 wait layer-0 MMAs, 1 layer-0 epilogue, 3 wait layer-1 MMAs, 4 last-layer epilogue, 5 outputs
+    // C: the consumer warpgroup works through every tile of this CTA; rows 64 h .. 64 h + 63 of a tile are half h.
+    // In the accumulator fragment this thread holds rows 64 h + 16 warp + g8 (+ 8) and columns 8 j + 2 c (+ 1).
+    // profile slots: 0 wait A tile, 1 layer 0, 2 layer 1, 3 last-layer epilogue + outputs
     // =====================================================================================================
-    const int g = warp >> 2, qd = warp & 3;
-    const int r = qd * WT + lane;  // tile row == TMEM lane
-    const uint32_t tb = tmem_base + g * WS_TCOLS;
-    const uint32_t tl = tb + ((uint32_t)(qd * 32) << 16);
-    const uint32_t bar0 = um_smem_u32(bars + WSB_MMA0 + g), bar1 = um_smem_u32(bars + WSB_MMA1 + g);
-    uint32_t ph0 = 0, ph1 = 0;
-    const int t = GRAD ? (lane & 3) : 0;  // row type: 0 value, 1..3 tangent d/dq_{t-1}
+    const int g8 = lane >> 2, c = lane & 3;
+    const int t = GRAD ? (g8 & 3) : 0;  // row type: 0 value, 1..3 tangent d/dq_{t-1}
     const float bsel = t == 0 ? 1.f : 0.f;
-    const int src = lane & ~3;  // the value row of this row's query
-    const float* s_b0 = reinterpret_cast<const float*>(sm + lay.b0);
+    const int src = lane & ~12;  // the lane holding the same columns of this row's value row
     const float* s_b1 = reinterpret_cast<const float*>(sm + lay.b1);
     const float* s_wout = reinterpret_cast<const float*>(sm + lay.wout);
     const float* s_bout = reinterpret_cast<const float*>(sm + lay.bout);
-    const uint32_t tl1 = L > 1 ? tl + 192 : tl;  // accumulator of the last hidden layer
-    const uint32_t a1_ready = um_smem_u32(bars + WSB_A1_READY + 4 * g), d1_free = um_smem_u32(bars + WSB_D1_FREE + g);
+    constexpr uint32_t A_SBO0 = (K0 / 4) * UM_A_LBO, W_SBO0 = (K0 / 4) * UM_W_LBO, W_SBO1 = (H / 4) * UM_W_LBO;
+    // a k-step (8 columns = two 16-byte chunks) advances the start-address field of a descriptor by 2 * LBO / 16
+    constexpr uint64_t A_STEP = (2 * UM_A_LBO) >> 4, W_STEP = (2 * UM_W_LBO) >> 4, A_HALF = (8 * A_SBO0) >> 4;
+    const uint64_t w0h_d = um_desc(um_smem_u32(sm + lay.w0_hi), UM_W_LBO, W_SBO0), w0l_d = um_desc(um_smem_u32(sm + lay.w0_lo), UM_W_LBO, W_SBO0);
+    const uint64_t w1h_d = um_desc(um_smem_u32(sm + lay.w1_hi), UM_W_LBO, W_SBO1), w1l_d = um_desc(um_smem_u32(sm + lay.w1_lo), UM_W_LBO, W_SBO1);
 
-    // bias (value rows) + ReLU gate of 16 accumulator columns.  The gate of a tangent row is the sign pattern of its
-    // query's value row: the 16 sign bits travel in ONE quad-leader shuffle per chunk.
-    auto gated16 = [&](const uint32_t (&v)[16], const float (&bb)[16], float (&z)[16]) {
+    // bias (value rows; `bias` may be null) + ReLU gate of the 32 accumulator values of a half.  The gate of a tangent
+    // row is the sign pattern of its query's value row: the 32 sign bits travel in ONE shuffle.
+    auto gate = [&](float (&z)[32], const float* bias) {
+      if (bias) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float2 b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * c);
+          z[4 * j] = fmaf(bsel, b.x, z[4 * j]);
+          z[4 * j + 1] = fmaf(bsel, b.y, z[4 * j + 1]);
+          z[4 * j + 2] = fmaf(bsel, b.x, z[4 * j + 2]);
+          z[4 * j + 3] = fmaf(bsel, b.y, z[4 * j + 3]);
+        }
+      }
       uint32_t mk = 0u;
 #pragma unroll
-      for (int e = 0; e < 16; ++e) {
-        z[e] = fmaf(bsel, bb[e], __uint_as_float(v[e]));
-        mk |= z[e] > 0.f ? (1u << e) : 0u;
-      }
+      for (int e = 0; e < 32; ++e) mk |= z[e] > 0.f ? (1u << e) : 0u;
       if (GRAD) mk = __shfl_sync(FULL, mk, src);
 #pragma unroll
-      for (int e = 0; e < 16; ++e) z[e] = ((mk >> e) & 1u) ? z[e] : slope * z[e];
+      for (int e = 0; e < 32; ++e) z[e] = ((mk >> e) & 1u) ? z[e] : slope * z[e];
     };
-
-    auto gate16 = [&](const uint32_t (&v)[16], float (&z)[16]) {  // gated16 without a bias
-      uint32_t mk = 0u;
+    // output head of the two rows of a half (quad-reduced: every lane of the quad holds the sums)
+    auto head = [&](const float (&z)[32], float (&o)[2][4]) {
 #pragma unroll
-      for (int e = 0; e < 16; ++e) {
-        z[e] = __uint_as_float(v[e]);
-        mk |= z[e] > 0.f ? (1u << e) : 0u;
+      for (int ch = 0; ch < 4; ++ch) {
+        o[0][ch] = o[1][ch] = 0.f;
+        if (ch < OC) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float2 w = *reinterpret_cast<const float2*>(s_wout + ch * H + 8 * j + 2 * c);
+            o[0][ch] = fmaf(z[4 * j + 1], w.y, fmaf(z[4 * j], w.x, o[0][ch]));
+            o[1][ch] = fmaf(z[4 * j + 3], w.y, fmaf(z[4 * j + 2], w.x, o[1][ch]));
+          }
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            o[r][ch] += __shfl_xor_sync(FULL, o[r][ch], 1);
+            o[r][ch] += __shfl_xor_sync(FULL, o[r][ch], 2);
+          }
+        }
       }
-      if (GRAD) mk = __shfl_sync(FULL, mk, src);
-#pragma unroll
-      for (int e = 0; e < 16; ++e) z[e] = ((mk >> e) & 1u) ? z[e] : slope * z[e];
     };
     // where this row's results go: element (query qi, channel ch) at out_base[qi * out_qstride + ch * out_chstride]
     float* out_base;
@@ -349,105 +291,114 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       out_qstride = p.is_color ? 3 * OC : 3;
       out_chstride = 3;
     }
-    for (long long T = blockIdx.x + (long long)g * gridDim.x; T < n_tiles; T += (long long)WS_EG * gridDim.x) {
-      ws_wait(bar0, ph0);
-      ph0 ^= 1u;
-      ws_fence_after();
-      clk.lap(0);
-      if (L > 1) {
-        // ---- layer-0 epilogue: gated activations, hi / lo split -> A1 in TMEM
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          uint32_t v[16];
-          float z[16];
-          um_tmem_ld16(tl + 16 * c, v);
-          gate16(v, z);  // the bias came through the MMA
-          uint32_t lo[16];
+    // value rows write the prediction, tangent rows one component of its gradient; lane c == r of the quad writes row r
+    auto store = [&](long long T, int h, float (&o)[2][4]) {
 #pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            v[e] = __float_as_uint(z[e]) & TF32_MASK;
-            lo[e] = __float_as_uint(z[e] - __uint_as_float(v[e]));
-          }
-          ws_tmem_st16(tl + 64 + 16 * c, v);
-          ws_tmem_st16(tl + 128 + 16 * c, lo);
-          // this row's 16 A1 columns are written (and its D0 columns read): the group's MMA warp starts the two
-          // k-steps of layer 1 that need them while the later chunks are still in the epilogue
-          asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-          ws_fence_before();
-          ws_arrive(a1_ready + 8 * c);
-        }
-        clk.lap(1);
-        ws_wait(bar1, ph1);
-        ph1 ^= 1u;
-        ws_fence_after();
-        clk.lap(3);
-      }
-      // ---- last hidden layer: gated activations, output head(s) in registers
-      float o[4] = {0.f, 0.f, 0.f, 0.f};
-      {
-        const float* bl = L > 1 ? s_b1 : s_b0;
-#pragma unroll 1
-        for (int c = 0; c < 2; ++c) {  // 32 columns per step: two TMEM loads and their bias rows in flight together
-          uint32_t va[16], vb[16];
-          float za[16], zb[16];
-          ws_tmem_ld16_issue(tl1 + 32 * c, va);
-          ws_tmem_ld16_issue(tl1 + 32 * c + 16, vb);
-          ws_lds16(bl + 32 * c, za);
-          ws_lds16(bl + 32 * c + 16, zb);
-          ws_tmem_ld_wait(va);
-          ws_tmem_ld_wait(vb);
-          gated16(va, za, za);
-          gated16(vb, zb, zb);
+      for (int r = 0; r < 2; ++r) {
+        if (p.dec.sigmoid_out) {
 #pragma unroll
           for (int ch = 0; ch < 4; ++ch)
             if (ch < OC) {
-              float wa[16], wb[16];
-              ws_lds16(s_wout + ch * H + 32 * c, wa);
-              ws_lds16(s_wout + ch * H + 32 * c + 16, wb);
-              float oa = 0.f, ob = 0.f;  // two independent chains
-#pragma unroll
-              for (int e = 0; e < 16; ++e) {
-                oa = fmaf(za[e], wa[e], oa);
-                ob = fmaf(zb[e], wb[e], ob);
-              }
-              o[ch] += oa + ob;
+              const float oo = fmaf(bsel, s_bout[ch], o[r][ch]);
+              const float val = 1.f / (1.f + expf(-oo));
+              const float dv = val * (1.f - val);
+              const float dvq = GRAD ? __shfl_sync(FULL, dv, src) : dv;
+              o[r][ch] = t == 0 ? val : dvq * oo;
             }
-        }
-      }
-      // this row has read its accumulator columns of the last layer
-      ws_fence_before();
-      ws_arrive(d1_free);
-      clk.lap(4);
-      // ---- outputs: value rows write the prediction, tangent rows one component of its gradient (destinations
-      // resolved once per thread, see out_base)
-      const long long qi = T * QT + (GRAD ? (r >> 2) : r);
-      if (p.dec.sigmoid_out) {
+        } else {
 #pragma unroll
-        for (int ch = 0; ch < 4; ++ch)
-          if (ch < OC) {
-            const float oo = fmaf(bsel, s_bout[ch], o[ch]);
-            const float val = 1.f / (1.f + expf(-oo));
-            const float dv = val * (1.f - val);
-            const float dvq = GRAD ? __shfl_sync(FULL, dv, src) : dv;
-            o[ch] = t == 0 ? val : dvq * oo;
+          for (int ch = 0; ch < 4; ++ch) o[r][ch] = fmaf(bsel, s_bout[ch], o[r][ch]) * p.dec.out_scale;
+        }
+        const int row = 64 * h + 16 * warp + g8 + 8 * r;
+        const long long qi = T * QT + (GRAD ? (row >> 2) : row);
+        if (c == r && qi < p.n) {
+          if (out_base) {
+            float* dst = out_base + qi * out_qstride;
+#pragma unroll
+            for (int ch = 0; ch < 4; ++ch)
+              if (ch < out_nch) dst[ch * out_chstride] = o[r][ch];
           }
-      } else {
-#pragma unroll
-        for (int ch = 0; ch < 4; ++ch) o[ch] = fmaf(bsel, s_bout[ch], o[ch]) * p.dec.out_scale;
-      }
-      if (qi < p.n) {
-        if (out_base) {
-          float* dst = out_base + qi * out_qstride;
-#pragma unroll
-          for (int ch = 0; ch < 4; ++ch)
-            if (ch < out_nch) dst[ch * out_chstride] = o[ch];
+          if (out_std) out_std[qi] = 0.f;
         }
-        if (out_std) out_std[qi] = 0.f;
       }
-      clk.lap(5);
+    };
+
+    int i = 0;
+    for (long long T = blockIdx.x; T < n_tiles; T += gridDim.x, ++i) {
+      const int slot = i % WS_A0;
+      ws_wait(um_smem_u32(bars + WSB_A0_FULL + slot), (uint32_t)(i / WS_A0) & 1u);
+      clk.lap(0);
+      // ---- layer 0: both halves, A tile from shared memory
+      float d0[2][32];
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 32; ++e) d0[h][e] = 0.f;
+      {
+        const uint32_t a_hi = um_smem_u32(sm + lay.a0 + slot * lay.a0_stride);
+        const uint64_t ah = um_desc(a_hi, UM_A_LBO, A_SBO0), al = um_desc(a_hi + lay.a0_half, UM_A_LBO, A_SBO0);
+        wg_fence();
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int s = 0; s < K0 / 8; ++s) {
+            wg_mma_n64(d0[h], al + h * A_HALF + s * A_STEP, w0h_d + s * W_STEP, s > 0);  // small terms first
+            wg_mma_n64(d0[h], ah + h * A_HALF + s * A_STEP, w0l_d + s * W_STEP, 1);
+            wg_mma_n64(d0[h], ah + h * A_HALF + s * A_STEP, w0h_d + s * W_STEP, 1);
+          }
+        wg_commit();
+        wg_wait0();
+      }
+      __syncwarp();
+      if (lane == 0) ws_arrive(um_smem_u32(bars + WSB_A0_EMPTY + slot));  // the gather team may refill the A tile
+      clk.lap(1);
+      float o[2][4];
+      if (L > 1) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          // ---- layer-0 epilogue (the bias came through the MMA): gated activations, hi / lo split in place -> layer 1
+          // with the A operand from registers
+          float d1[32];
+          uint32_t lo[32];
+#pragma unroll
+          for (int e = 0; e < 32; ++e) d1[e] = 0.f;
+          gate(d0[h], nullptr);
+#pragma unroll
+          for (int e = 0; e < 32; ++e) {
+            const float hi = __uint_as_float(__float_as_uint(d0[h][e]) & TF32_MASK);
+            lo[e] = __float_as_uint(d0[h][e] - hi);
+            d0[h][e] = hi;
+          }
+          wg_fence();
+#pragma unroll
+          for (int s = 0; s < H / 8; ++s) {
+            const uint32_t h0 = __float_as_uint(d0[h][4 * s]), h1 = __float_as_uint(d0[h][4 * s + 2]),
+                           h2 = __float_as_uint(d0[h][4 * s + 1]), h3 = __float_as_uint(d0[h][4 * s + 3]);
+            wg_mma_n64_rs(d1, lo[4 * s], lo[4 * s + 2], lo[4 * s + 1], lo[4 * s + 3], w1h_d + s * W_STEP, s > 0);
+            wg_mma_n64_rs(d1, h0, h1, h2, h3, w1l_d + s * W_STEP, 1);
+            wg_mma_n64_rs(d1, h0, h1, h2, h3, w1h_d + s * W_STEP, 1);
+          }
+          wg_commit();
+          wg_wait0();
+          clk.lap(2);
+          // ---- last hidden layer: bias, gate, output head(s), results
+          gate(d1, s_b1);
+          head(d1, o);
+          store(T, h, o);
+        }
+      } else {
+        // single hidden layer: its bias came through the MMA
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          gate(d0[h], nullptr);
+          head(d0[h], o);
+          store(T, h, o);
+        }
+      }
+      clk.lap(3);
     }
-  } else if (warp < 4 * WS_EG + WS_GT * WS_GW) {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(WS_REG_G));
+  } else if (warp < WS_CW + WS_GT * WS_GW) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(WS_REG_G));
     // =====================================================================================================
     // G: gather teams -- the 4 warps of a team work on the same tile, each on its share of the queries: per round a
     // lane has GU passes x K feature-row loads (16 x LDG.128 for F = 32) in flight; the two teams (and the ring of A
@@ -456,7 +407,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
     // profile slots: 0 wait free A tile, 1 wait meta block, 2 feature-row loads issued, 3 reduce + A-tile stores,
     //                4 position rows + fence + arrive
     // =====================================================================================================
-    const int team = (warp - 4 * WS_EG) / WS_GW, gw = (warp - 4 * WS_EG) % WS_GW;
+    const int team = (warp - WS_CW) / WS_GW, gw = (warp - WS_CW) % WS_GW;
     const int sub = lane / M::LPR, c4 = lane % M::LPR;
     const float4* __restrict__ f4 = reinterpret_cast<const float4*>(p.feat) + c4;
     constexpr int GU = NPASS / WS_GW >= 2 ? 2 : 1;  // passes in flight per gather warp
@@ -562,7 +513,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
             *reinterpret_cast<float4*>(a_lo + off) = make_float4(0.f, 0.f, 0.f, 0.f);
           }
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // A-tile writes -> visible to the tensor core
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // A-tile writes -> visible to wgmma
         __syncwarp();
         if (lane == 0) ws_arrive(um_smem_u32(bars + WSB_META_EMPTY + ms));
         clk.lap(4);
@@ -570,86 +521,14 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       if (lane == 0) ws_arrive(um_smem_u32(bars + WSB_A0_FULL + slot));
     }
   } else {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(WS_REG_L));  // one call site for the whole 4-warp group
-    if (warp >= 4 * WS_EG + WS_GT * WS_GW + WS_LW) {
-    // =====================================================================================================
-    // M: one MMA warp per epilogue group (lane 0 issues).  Software pipeline over the group's tiles: layer 0 of tile
-    // t+1 goes right behind layer 1 of tile t (separate accumulator columns), so it runs under the last-layer
-    // epilogue of tile t.  With the issue loop on its own warp the epilogue warps are never blocked by a full
-    // tensor-pipe queue (the group's first warp was: 3.8k of 11.5k cycles per tile, profiles/r02_k1_wsq_*).
-    // profile slots: 0 wait A1 / D0, 1 wait D1 free, 2 layer-1 issue, 3 wait A tile, 4 layer-0 issue
-    // =====================================================================================================
-    const int g = warp - (4 * WS_EG + WS_GT * WS_GW + WS_LW);
-    const uint32_t tb = tmem_base + g * WS_TCOLS;
-    const uint32_t bar0 = um_smem_u32(bars + WSB_MMA0 + g), bar1 = um_smem_u32(bars + WSB_MMA1 + g);
-    const uint32_t a1_ready = um_smem_u32(bars + WSB_A1_READY + 4 * g), d1_free = um_smem_u32(bars + WSB_D1_FREE + g);
-    constexpr uint32_t A_SBO0 = (K0 / 4) * UM_A_LBO, W_SBO0 = (K0 / 4) * UM_W_LBO, W_SBO1 = (H / 4) * UM_W_LBO;
-    // a k-step (8 columns = two 16-byte chunks) advances the start-address field of a descriptor by 2 * LBO / 16
-    constexpr uint64_t A_STEP = (2 * UM_A_LBO) >> 4, W_STEP = (2 * UM_W_LBO) >> 4;
-    const uint64_t w0h_d = um_desc(um_smem_u32(sm + lay.w0_hi), UM_W_LBO, W_SBO0), w0l_d = um_desc(um_smem_u32(sm + lay.w0_lo), UM_W_LBO, W_SBO0);
-    const uint64_t w1h_d = um_desc(um_smem_u32(sm + lay.w1_hi), UM_W_LBO, W_SBO1), w1l_d = um_desc(um_smem_u32(sm + lay.w1_lo), UM_W_LBO, W_SBO1);
-    const uint32_t idesc = um_idesc(H);
-    const uint32_t td1 = L > 1 ? tb + 192 : tb;  // accumulator of the last hidden layer
-    auto issue_l0 = [&](int ii) {  // layer 0 of the CTA's ii-th tile
-      const int slot = ii % WS_A0;
-      ws_wait(um_smem_u32(bars + WSB_A0_FULL + slot), (uint32_t)(ii / WS_A0) & 1u);
-      clk.lap(3);
-      if (ws_elect()) {
-        ws_fence_after();
-        const uint32_t a_hi = um_smem_u32(sm + lay.a0 + slot * lay.a0_stride);
-        const uint64_t ah = um_desc(a_hi, UM_A_LBO, A_SBO0), al = um_desc(a_hi + lay.a0_half, UM_A_LBO, A_SBO0);
-#pragma unroll
-        for (int s = 0; s < K0 / 8; ++s) {
-          um_mma(tb, al + s * A_STEP, w0h_d + s * W_STEP, idesc, s > 0);  // small terms first
-          um_mma(tb, ah + s * A_STEP, w0l_d + s * W_STEP, idesc, 1);
-          um_mma(tb, ah + s * A_STEP, w0h_d + s * W_STEP, idesc, 1);
-        }
-        ws_commit(bar0);
-        ws_commit(um_smem_u32(bars + WSB_A0_EMPTY + slot));  // the A tile may be refilled once these MMAs have read it
-      }
-      __syncwarp();
-      clk.lap(4);
-    };
-    int i = g;
-    uint32_t n = 0;  // tiles of this group so far
-    long long T = blockIdx.x + (long long)g * gridDim.x;
-    if (T < n_tiles) issue_l0(i);
-    for (; T < n_tiles; T += (long long)WS_EG * gridDim.x, i += WS_EG, ++n) {
-      const bool has_next = T + (long long)WS_EG * gridDim.x < n_tiles;
-      if (L > 1) {
-        if (n > 0) ws_wait(d1_free, (n - 1u) & 1u);  // every row has read the previous tile's last accumulator
-        clk.lap(1);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {  // layer 1 follows the layer-0 epilogue chunk by chunk (16 A1 columns = 2 k-steps)
-          ws_wait(a1_ready + 8 * c, n & 1u);
-          clk.lap(0);
-          if (ws_elect()) {
-            ws_fence_after();
-#pragma unroll
-            for (int s = 2 * c; s < 2 * c + 2; ++s) {
-              ws_mma_ts(td1, tb + 128 + 8 * s, w1h_d + s * W_STEP, idesc, s > 0);
-              ws_mma_ts(td1, tb + 64 + 8 * s, w1l_d + s * W_STEP, idesc, 1);
-              ws_mma_ts(td1, tb + 64 + 8 * s, w1h_d + s * W_STEP, idesc, 1);
-            }
-            if (c == 3) ws_commit(bar1);
-          }
-          __syncwarp();
-          clk.lap(2);
-        }
-      } else {
-        ws_wait(d1_free, n & 1u);  // single hidden layer: the epilogue reads the layer-0 accumulator itself
-        clk.lap(1);
-      }
-      if (has_next) issue_l0(i + WS_EG);
-    }
-    } else {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(WS_REG_L));
     // =====================================================================================================
     // L: loader warps -- TMA bulk copies of the search launch's results into the meta ring: neighbour ids + IDW weights
     // (2 KB), position part (384 B) and, with d/dq, the forward-mode seeds (4.1 KB) of a 32-query block, all counted in
     // bytes on the block's "full" mbarrier.  No thread touches the data.
     // profile slots: 0 wait free meta block, 1 copies issued
     // =====================================================================================================
-    const int lw = warp - 4 * WS_EG - WS_GT * WS_GW;
+    const int lw = warp - WS_CW - WS_GT * WS_GW;
     // the only role that reads what the search launch wrote: with programmatic dependent launch this grid may have
     // started before that one finished
     asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -684,13 +563,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       }
     }
   }
-  }
   clk.flush(warp);
-
-  // ---- teardown
-  ws_fence_before();
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
 }
 
 // ---------------------------------------------------------------------------
@@ -724,7 +597,6 @@ static WsLayout plan_ws_layout(const pinb200_decoder_view& d, bool grad) {
   l.n_meta = grad ? 8 : 16;
   l.meta = take(l.n_meta * l.meta_stride);
   l.bars = take(WSB_COUNT * 8);
-  l.tmem = take(4);
   l.total = o;
   return l;
 }
@@ -793,7 +665,7 @@ int dispatch_wsq(QueryParams& p, cudaStream_t stream) {
 
 void wsq_set_profile(int on) { g_ws_profile = on; }
 
-// copies the cycle counters of the last profiled launch: [148 CTAs][20 warps][8 slots] uint64
+// copies the cycle counters of the last profiled launch: [WS_PROF_CTAS CTAs][16 warps][8 slots] uint64
 int wsq_read_profile(unsigned long long* host_out, int64_t count) {
   const int64_t have = (int64_t)(sizeof(g_ws_prof) / sizeof(unsigned long long));
   if (count < have) {

@@ -1,4 +1,4 @@
-"""Make the reference's own import statements resolve to the B200 drop-ins.
+"""Make the reference's own import statements resolve to the CUDA drop-ins.
 
 `pin_slam.py` (and utils/tracker.py, utils/mapper.py, utils/mesher.py ...) of the
 reference import `from model.neural_points import NeuralPoints` and

@@ -1,10 +1,10 @@
-"""Drop-in `NeuralPoints` for PIN-SLAM backed by the sm_100a kernels.
+"""Drop-in `NeuralPoints` for PIN-SLAM backed by the sm_90a kernels.
 
 Keeps the Python surface of the reference class (model/neural_points.py:29 of
 PRBonn/PIN_SLAM: constructor, tensor attribute names, method names, argument
 meaning, return tuples) so that `pin_slam.py` and the reference's tracker /
 mapper / mesher / GUI code run against it unchanged, and adds the fused entry
-points the B200 tracker / mapper use:
+points the CUDA tracker / mapper use:
 
     query_sdf(...)        one launch: voxel-hash kNN + IDW + decoder (+ d/dx)   [K1]
     map_handle(...)       the plain-C view of the map handed to the kernels
@@ -37,6 +37,17 @@ def _quat_rotate_passive(quat, v):
     u = -quat[..., 1:]
     t = 2.0 * torch.linalg.cross(u, v)
     return v + w * t + torch.linalg.cross(u, t)
+
+
+def _put_last(table: torch.Tensor, slots: torch.Tensor, vals: torch.Tensor) -> None:
+    """table[slots] = vals with sequential semantics: where a slot repeats, the last write wins.  A plain index_put
+    with duplicate indices leaves the winner unspecified (on the CPU it depends on the thread count)."""
+    slots = slots.long()
+    pos = torch.arange(slots.numel(), device=slots.device)
+    last = torch.full(table.shape, -1, dtype=torch.int64, device=slots.device)
+    last.scatter_reduce_(0, slots, pos, reduce="amax")
+    keep = last[slots] == pos
+    table[slots[keep]] = vals[keep]
 
 
 def voxel_down_sample(points: torch.Tensor, voxel_size: float) -> torch.Tensor:
@@ -702,7 +713,7 @@ class NeuralPoints(nn.Module):
             score = self.point_certainties.max() - self.point_certainties
         pick = voxel_down_sample_min_value(self.neural_points, res, score)
         if kept_points:
-            self.buffer_pt_index[self._slots(self.neural_points[pick])] = pick.to(torch.int32)
+            _put_last(self.buffer_pt_index, self._slots(self.neural_points[pick]), pick.to(torch.int32))
         else:
             if not self.silence:
                 print("Filter duplicated neural points")
@@ -716,8 +727,8 @@ class NeuralPoints(nn.Module):
             if self.color_features is not None:
                 self.color_features = self.color_features[pick_pad]
             n = self.neural_points.shape[0]
-            self.buffer_pt_index[self._slots(self.neural_points)] = torch.arange(n, dtype=torch.int32,
-                                                                                device=self.device)
+            _put_last(self.buffer_pt_index, self._slots(self.neural_points),
+                      torch.arange(n, dtype=torch.int32, device=self.device))
         self._invalidate(slots_freed=True)
         if sensor_position is not None:
             self.reset_local_map(sensor_position, sensor_orientation, cur_ts)

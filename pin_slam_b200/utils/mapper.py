@@ -449,7 +449,7 @@ class Mapper:
         """Reference: utils/mapper.py:600-844."""
         cfg = self.config
         if not (cfg.main_loss_type == "bce" and cfg.numerical_grad and cfg.opt_adam):
-            raise NotImplementedError("B200 mapper supports the reference defaults: bce loss, numerical Eikonal, Adam")
+            raise NotImplementedError("the CUDA mapper supports the reference defaults: bce loss, numerical Eikonal, Adam")
         iter_count = max(1, iter_count + self.adaptive_iter_offset)
         npm = self.neural_points
         feat = npm.local_geo_features.data
@@ -593,4 +593,4 @@ class Mapper:
         return n
 
     def bundle_adjustment(self, iter_count, window_size: int = 50, use_lie_group: bool = False):
-        raise NotImplementedError("local bundle adjustment (pypose) is outside the B200 hot path (SURVEY.md section 2 #4)")
+        raise NotImplementedError("local bundle adjustment (pypose) is outside the CUDA hot path (SURVEY.md section 2 #4)")

@@ -31,7 +31,7 @@ class Mesher:
         compatibility (it only sets a lower bound on the chunk size, the kernel takes millions of points per
         launch)."""
         if query_sem:
-            raise NotImplementedError("semantic head is outside the B200 hot path")
+            raise NotImplementedError("semantic head is outside the CUDA hot path")
         n = coord.shape[0]
         dev = self.neural_points.neural_points.device
         chunk = max(int(bs), self.CHUNK)

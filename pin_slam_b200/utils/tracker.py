@@ -46,7 +46,7 @@ class Tracker:
         """Same outputs as the reference (utils/tracker.py:227-365); `bs` is accepted for compatibility,
         the fused kernel takes the whole batch in one launch."""
         if query_sem:
-            raise NotImplementedError("semantic head is outside the B200 hot path")
+            raise NotImplementedError("semantic head is outside the CUDA hot path")
         color_dec = self.color_mlp if query_color else None
         o = self.neural_points.query_sdf(coord.contiguous(), self.sdf_mlp, query_locally=query_locally,
                                          need_grad=query_sdf_grad or query_color_grad, color_decoder=color_dec,

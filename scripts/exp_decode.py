@@ -67,9 +67,9 @@ ops.set_option("ws_profile", 1)
 npm.query_sdf(q, dec, out=out)
 torch.cuda.synchronize()
 ops.set_option("ws_profile", 0)
-buf = np.zeros(148 * 20 * 8, dtype=np.uint64)
+buf = np.zeros(132 * 16 * 8, dtype=np.uint64)
 _lib.check(_lib.load().pinb200_debug_read(b"ws_profile", buf.ctypes.data, buf.size), "debug_read")
-prof = buf.reshape(148, 20, 8).astype(np.float64)
+prof = buf.reshape(132, 16, 8).astype(np.float64)
 names = {"E": ["wait_mma0", "epi0", "-", "wait_mma1", "epi1", "outputs"], "M": ["wait_A1", "wait_D1free", "issue_L1", "wait_Atile", "issue_L0"], "G": ["wait_A_free", "wait_meta", "issue_loads", "reduce+store", "pos+fence"],
          "L": ["wait_meta_free", "stash_loads", "seeds+store"]}
 for role, ws in (("E", range(0, 8)), ("G", range(8, 16)), ("L", range(16, 18)), ("M", range(18, 20))):

@@ -1,5 +1,5 @@
 // Microbenchmark: random 16-byte gathers (one sector per lane) -- achievable sectors/cycle/SM vs resident warps and
-// loads in flight per thread, for an L2-resident and a DRAM-resident table.   nvcc -arch=sm_100a -O3 -o gather_bw gather_bw.cu
+// loads in flight per thread, for an L2-resident and a DRAM-resident table.   nvcc -arch=sm_90a -O3 -o gather_bw gather_bw.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -133,7 +133,7 @@ def test_cuda_tracking_loop_matches_reference():
     dT = np.abs(T.cpu().numpy() - fx["result.T"])
     print(f"[tracking] {len(log)} iterations, max |dT| rot {dT[:3, :3].max():.2e} trans {dT[:3, 3].max():.2e} m, "
           f"max residual dev {np.abs(res - fx['result.residual_cm']).max():.2e} cm")
-    # SURVEY.md 8(c): <= 1e-6 m / 1e-7 rad per GN step; measured on the B200 after 18 chained steps: 2.3e-7 m, 3.4e-8
+    # SURVEY.md 8(c): <= 1e-6 m / 1e-7 rad per GN step, bounded here over all chained steps of the loop
     assert dT[:3, 3].max() <= 2e-6 and dT[:3, :3].max() <= 5e-7
 
 
@@ -339,7 +339,7 @@ def test_unchanged_reference_tracker_runs_fused():
 
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     if not os.path.isfile(os.path.join(root, "oracle", "_ref", "utils", "tracker.py")):
-        pytest.skip("oracle/_ref not vendored (built by __graft_entry__.build() where /root/reference exists)")
+        pytest.skip("oracle/_ref not built: oracle/make_ref.py needs a checkout of the original PIN-SLAM")
     pr = subprocess.run([sys.executable, os.path.join(root, "tests", "unchanged_caller_check.py")], capture_output=True,
                         text=True, timeout=600)
     assert pr.returncode == 0, pr.stdout[-2000:] + pr.stderr[-4000:]

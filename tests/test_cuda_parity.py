@@ -232,7 +232,7 @@ def test_fused_query_vs_oracle_synthetic(F, K, L, wf, pgo, C):
                                                    (16, 4, 2, True, False, False), (32, 8, 1, True, True, True),
                                                    (8, 3, 2, False, False, True)])
 def test_split_pipeline_decoders_vs_oracle(F, K, L, pgo, color, leaky, variant):
-    """The two-launch pipeline (search_kernel -> tcgen05 decode) forced onto oracle-sized batches: the
+    """The two-launch pipeline (search_kernel -> tensor-core decode) forced onto oracle-sized batches: the
     warp-specialised forward-mode decode (variant 1, default) and the phase-synchronous decode with backward MMAs
     (variant 0) against the oracle -- value, d/dq, colour head + its Jacobian, ragged last tile, queries without
     neighbours, and the value-only launch (128-query tiles)."""
@@ -721,7 +721,7 @@ def test_dropin_query_feature_matches_fused_path():
 def test_host_facing_pipelined_query_equals_device_query():
     """NeuralPoints.query_sdf_host (pinned host in/out, pieces pipelined over two streams) returns what the
     device-resident call returns, for ragged piece sizes too: bit for bit when both run the same kernels; when the
-    device call is large enough for the split search + tcgen05 decode pipeline while the host pieces are not, the
+    device call is large enough for the split search + tensor-core decode pipeline while the host pieces are not, the
     search outputs stay bit-identical and the decoder outputs agree within the 3xTF32 parity bound."""
     from pin_slam_b200.config import HotPathConfig
     from pin_slam_b200.model import Decoder

@@ -74,6 +74,33 @@ __device__ __forceinline__ void wg_mma_n64_rs(float (&d)[32], uint32_t a0, uint3
       : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(acc)
       : "memory");
 }
+// The same two MMAs with the descriptors advanced by compile-time k-step offsets inside the asm statement: the caller
+// keeps one base descriptor per operand live instead of one (uniform) register pair per k-step, which is what a
+// 136-register warpgroup can afford.
+template <int AOFF, int BOFF>
+__device__ __forceinline__ void wg_mma_n64_at(float (&d)[32], uint64_t adesc, uint64_t bdesc, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b64 ad, bd;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "add.s64 ad, %32, %35;\n\t"
+      "add.s64 bd, %33, %36;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " PINB_WG_D32 ", ad, bd, p, 1, 1;\n\t}\n"
+      : PINB_WG_D32_OPS
+      : "l"(adesc), "l"(bdesc), "r"(acc), "n"(AOFF), "n"(BOFF)
+      : "memory");
+}
+template <int BOFF>
+__device__ __forceinline__ void wg_mma_n64_rs_at(float (&d)[32], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
+                                                 uint64_t bdesc, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b64 bd;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "add.s64 bd, %36, %38;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " PINB_WG_D32 ", {%32, %33, %34, %35}, bd, p, 1, 1;\n\t}\n"
+      : PINB_WG_D32_OPS
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(acc), "n"(BOFF)
+      : "memory");
+}
 #undef PINB_WG_D32
 #undef PINB_WG_D32_OPS
 

@@ -1,18 +1,20 @@
 // K1b, warp-specialised: gather + decoder + d/dq of the split pipeline for weighted_first maps, as ONE persistent CTA
 // per SM whose warps have different jobs and only meet through mbarriers (no block-wide barrier after the prologue):
 //
-//   L  loader warps   TMA bulk copies (cp.async.bulk, completion counted in bytes on an mbarrier) of what search_kernel
-//                     wrote for a 32-query block -- neighbour ids, IDW weights, position part of the decoder input and,
-//                     when d/dq is wanted, the forward-mode seeds  omega_kj = d w_k / d q_j  and d(position part)/dq --
-//                     into a ring of "meta" blocks in shared memory; no thread touches the data
-//   G  gather teams   (2 x 4 warps, 120 registers) F/4 lanes per feature row (a 128-byte row = 8 lanes x LDG.128): ONE pass
-//                     over the K rows gives the IDW-interpolated feature  xbar = sum_k w_k f_k  AND its three directional
+//   G  gather teams   (2 x 4 warps, 120 registers) TMA bulk copies (cp.async.bulk, completion counted in bytes on an
+//                     mbarrier) of what search_kernel wrote for a 32-query block -- neighbour ids, IDW weights, position
+//                     part of the decoder input and, when d/dq is wanted, the forward-mode seeds  omega_kj = d w_k / d q_j
+//                     and d(position part)/dq -- into a ring of "meta" blocks in shared memory, issued by one lane a few
+//                     blocks ahead; then F/4 lanes per feature row (a 128-byte row = 8 lanes x LDG.128): ONE pass over the
+//                     K rows gives the IDW-interpolated feature  xbar = sum_k w_k f_k  AND its three directional
 //                     derivatives  T_j = sum_k omega_kj (f_k - f_0)  -> rows of an A tile (canonical K-major, hi / lo TF32)
-//   C  consumer       (one warpgroup, 216 registers) layer 0 as wgmma.mma_async with the A tile from shared memory (two
-//                     64-row halves, accumulators in registers), then releases the A tile to its gather team; ReLU gate,
-//                     hi / lo split in registers, layer 1 with the A operand IN REGISTERS (the accumulator fragment is the
-//                     A fragment once the k order inside a k-step is permuted, see um_kperm: the layer-1 weights are staged
-//                     in that order); last layer: output head in registers (quad shuffles), results to global memory.
+//   C  consumers      (2 warpgroups, 136 registers; warpgroup h owns the 64-row half h of every tile) layer 0 as
+//                     wgmma.mma_async with the A tile from shared memory (accumulators in registers), then releases the A
+//                     tile to its gather team; ReLU gate, hi / lo split in registers, layer 1 with the A operand IN
+//                     REGISTERS (the accumulator fragment is the A fragment once the k order inside a k-step is permuted,
+//                     see um_kperm: the layer-1 weights are staged in that order); last layer: output head in registers
+//                     (quad shuffles), results to global memory.  The two warpgroups drift apart, so one's MMA waits run
+//                     under the other's epilogue.
 //
 // d sdf / d q is computed in FORWARD mode: a tile row is either a value row (decoder input x) or one of the three
 // tangent rows (dx / dq_j) of the same query; tangent rows go through the same weights, without bias, and are gated
@@ -29,15 +31,15 @@
 
 namespace pinb {
 
-constexpr int WS_CW = 4;       // consumer warps (one warpgroup)
+constexpr int WS_CG = 2;       // consumer warpgroups: warpgroup h owns rows 64 h .. 64 h + 63 (half h) of every tile
+constexpr int WS_CW = 4 * WS_CG;  // consumer warps
 constexpr int WS_GT = 2;       // gather teams of 4 warps: team t fills the A tiles of the CTA's tiles i = t (mod WS_GT)
 constexpr int WS_GW = 4;       // warps per gather team
-constexpr int WS_LW = 4;       // loader warps
-constexpr int WS_THREADS = (WS_CW + WS_GT * WS_GW + WS_LW) * 32;
+constexpr int WS_THREADS = (WS_CW + WS_GT * WS_GW) * 32;
 // register budget per thread (setmaxnreg, one value per 4-warp group).  The pool is what the CTA was launched with
 // (512 threads x 128 registers)
-constexpr int WS_REG_C = 216, WS_REG_G = 120, WS_REG_L = 56;
-static_assert((WS_CW * WS_REG_C + WS_GT * WS_GW * WS_REG_G + WS_LW * WS_REG_L) * 32 <= WS_THREADS * 128, "setmaxnreg pool");
+constexpr int WS_REG_C = 136, WS_REG_G = 120;
+static_assert((WS_CW * WS_REG_C + WS_GT * WS_GW * WS_REG_G) * 32 <= WS_THREADS * 128, "setmaxnreg pool");
 constexpr int WS_A0 = 2;       // A-tile ring slots, one per gather team
 
 struct WsMeta {  // float offsets inside a meta block of 32 queries, [field][k][lane]
@@ -61,10 +63,14 @@ constexpr int WS_MB_MAX = 16;
 constexpr int WSB_A0_FULL = 0, WSB_A0_EMPTY = WSB_A0_FULL + WS_A0, WSB_META_FULL = WSB_A0_EMPTY + WS_A0,
               WSB_META_EMPTY = WSB_META_FULL + WS_MB_MAX, WSB_COUNT = WSB_META_EMPTY + WS_MB_MAX;
 
-// Optional cycle accounting (pinb200_set_option("ws_profile", 1)): per warp, clock deltas of up to 8 phases,
+// Optional cycle accounting (pinb200_set_option("ws_profile", 1)): per warp, clock deltas of up to 7 phases,
 // summed over the tiles of the launch, for the first WS_PROF_CTAS CTAs; read back with
-// pinb200_debug_read("ws_profile", ...).
+// pinb200_debug_read("ws_profile", ...).  The last slot of every warp holds its role code (WS_ROLE_*), so that a
+// reader of the counters (scripts/exp_decode.py) follows the kernel's role layout.
 constexpr int WS_PROF_SLOTS = 8;
+// C consumer warps, G gather warps that also fill the meta ring (codes 2 and 3 stood for gather-only warps and
+// separate loader warps, an earlier layout that exp_decode.py still reads)
+constexpr int WS_ROLE_C = 1, WS_ROLE_G = 4;
 constexpr int WS_PROF_CTAS = 132;  // one CTA per SM of an H100 SXM
 __device__ unsigned long long g_ws_prof[WS_PROF_CTAS * (WS_THREADS / 32) * WS_PROF_SLOTS];
 static int g_ws_profile = 0;
@@ -87,11 +93,13 @@ struct WsClock {  // PROF = false: no code at all (64-bit counters in the produc
       last = now;
     }
   }
-  __device__ __forceinline__ void flush(int warp) {
+  __device__ __forceinline__ void flush(int warp, int role) {
     if (PROF) {
       if ((threadIdx.x & 31) == 0 && blockIdx.x < WS_PROF_CTAS) {
+        unsigned long long* dst = g_ws_prof + (blockIdx.x * (WS_THREADS / 32) + warp) * WS_PROF_SLOTS;
 #pragma unroll
-        for (int i = 0; i < WS_PROF_SLOTS; ++i) g_ws_prof[(blockIdx.x * (WS_THREADS / 32) + warp) * WS_PROF_SLOTS + i] = acc[i];
+        for (int i = 0; i < WS_PROF_SLOTS - 1; ++i) dst[i] = acc[i];
+        dst[WS_PROF_SLOTS - 1] = (unsigned long long)role;
       }
     }
   }
@@ -136,6 +144,16 @@ __device__ __forceinline__ void ws_arrive(uint32_t bar) {
 
 static_assert(WsMeta::P - WsMeta::om == Seeds::P - Seeds::om && WsMeta::floats_g - WsMeta::om == Seeds::floats,
               "the seed block of the search launch is copied verbatim into the meta block");
+
+// fn(std::integral_constant<int, s>) for s = 0 .. N-1: a k-step loop whose step is a compile-time constant
+template <typename Fn, int... S>
+__device__ __forceinline__ void ws_unroll_seq(Fn&& fn, std::integer_sequence<int, S...>) {
+  (fn(std::integral_constant<int, S>{}), ...);
+}
+template <int N, typename Fn>
+__device__ __forceinline__ void ws_unroll(Fn&& fn) {
+  ws_unroll_seq(fn, std::make_integer_sequence<int, N>{});
+}
 
 __device__ __forceinline__ bool ws_elect() {  // one lane of the (converged) warp; keeps the code warp-uniform for the compiler
   uint32_t pred;
@@ -219,10 +237,13 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
   if (warp < WS_CW) {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(WS_REG_C));
     // =====================================================================================================
-    // C: the consumer warpgroup works through every tile of this CTA; rows 64 h .. 64 h + 63 of a tile are half h.
-    // In the accumulator fragment this thread holds rows 64 h + 16 warp + g8 (+ 8) and columns 8 j + 2 c (+ 1).
+    // C: both consumer warpgroups work through every tile of this CTA; warpgroup h takes rows 64 h .. 64 h + 63 of a
+    // tile (half h), so one warpgroup's MMA waits run under the other's epilogue.  The four rows of a query lie in
+    // the same half.  In the accumulator fragment this thread holds rows 64 h + 16 wq + g8 (+ 8) and columns
+    // 8 j + 2 c (+ 1).
     // profile slots: 0 wait A tile, 1 layer 0, 2 layer 1, 3 last-layer epilogue + outputs
     // =====================================================================================================
+    const int h = warp / 4, wq = warp % 4;
     const int g8 = lane >> 2, c = lane & 3;
     const int t = GRAD ? (g8 & 3) : 0;  // row type: 0 value, 1..3 tangent d/dq_{t-1}
     const float bsel = t == 0 ? 1.f : 0.f;
@@ -256,7 +277,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
 #pragma unroll
       for (int e = 0; e < 32; ++e) z[e] = ((mk >> e) & 1u) ? z[e] : slope * z[e];
     };
-    // output head of the two rows of a half (quad-reduced: every lane of the quad holds the sums)
+    // output head of the two rows of this thread (quad-reduced: every lane of the quad holds the sums)
     auto head = [&](const float (&z)[32], float (&o)[2][4]) {
 #pragma unroll
       for (int ch = 0; ch < 4; ++ch) {
@@ -292,7 +313,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       out_chstride = 3;
     }
     // value rows write the prediction, tangent rows one component of its gradient; lane c == r of the quad writes row r
-    auto store = [&](long long T, int h, float (&o)[2][4]) {
+    auto store = [&](long long T, float (&o)[2][4]) {
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         if (p.dec.sigmoid_out) {
@@ -309,7 +330,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
 #pragma unroll
           for (int ch = 0; ch < 4; ++ch) o[r][ch] = fmaf(bsel, s_bout[ch], o[r][ch]) * p.dec.out_scale;
         }
-        const int row = 64 * h + 16 * warp + g8 + 8 * r;
+        const int row = 64 * h + 16 * wq + g8 + 8 * r;
         const long long qi = T * QT + (GRAD ? (row >> 2) : row);
         if (c == r && qi < p.n) {
           if (out_base) {
@@ -328,24 +349,20 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       const int slot = i % WS_A0;
       ws_wait(um_smem_u32(bars + WSB_A0_FULL + slot), (uint32_t)(i / WS_A0) & 1u);
       clk.lap(0);
-      // ---- layer 0: both halves, A tile from shared memory
-      float d0[2][32];
+      // ---- layer 0 of this warpgroup's half, A tile from shared memory
+      float d0[32];
 #pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int e = 0; e < 32; ++e) d0[h][e] = 0.f;
+      for (int e = 0; e < 32; ++e) d0[e] = 0.f;
       {
         const uint32_t a_hi = um_smem_u32(sm + lay.a0 + slot * lay.a0_stride);
-        const uint64_t ah = um_desc(a_hi, UM_A_LBO, A_SBO0), al = um_desc(a_hi + lay.a0_half, UM_A_LBO, A_SBO0);
+        const uint64_t ah = um_desc(a_hi, UM_A_LBO, A_SBO0) + h * A_HALF, al = um_desc(a_hi + lay.a0_half, UM_A_LBO, A_SBO0) + h * A_HALF;
         wg_fence();
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int s = 0; s < K0 / 8; ++s) {
-            wg_mma_n64(d0[h], al + h * A_HALF + s * A_STEP, w0h_d + s * W_STEP, s > 0);  // small terms first
-            wg_mma_n64(d0[h], ah + h * A_HALF + s * A_STEP, w0l_d + s * W_STEP, 1);
-            wg_mma_n64(d0[h], ah + h * A_HALF + s * A_STEP, w0h_d + s * W_STEP, 1);
-          }
+        ws_unroll<K0 / 8>([&](auto S) {
+          constexpr int s = decltype(S)::value, AO = s * A_STEP, WO = s * W_STEP;
+          wg_mma_n64_at<AO, WO>(d0, al, w0h_d, s > 0);  // small terms first
+          wg_mma_n64_at<AO, WO>(d0, ah, w0l_d, 1);
+          wg_mma_n64_at<AO, WO>(d0, ah, w0h_d, 1);
+        });
         wg_commit();
         wg_wait0();
       }
@@ -354,71 +371,111 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       clk.lap(1);
       float o[2][4];
       if (L > 1) {
+        // ---- layer-0 epilogue (the bias came through the MMA): gated activations, hi / lo split in place -> layer 1
+        // with the A operand from registers
+        float d1[32];
+        uint32_t lo[32];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          // ---- layer-0 epilogue (the bias came through the MMA): gated activations, hi / lo split in place -> layer 1
-          // with the A operand from registers
-          float d1[32];
-          uint32_t lo[32];
+        for (int e = 0; e < 32; ++e) d1[e] = 0.f;
+        gate(d0, nullptr);
 #pragma unroll
-          for (int e = 0; e < 32; ++e) d1[e] = 0.f;
-          gate(d0[h], nullptr);
-#pragma unroll
-          for (int e = 0; e < 32; ++e) {
-            const float hi = __uint_as_float(__float_as_uint(d0[h][e]) & TF32_MASK);
-            lo[e] = __float_as_uint(d0[h][e] - hi);
-            d0[h][e] = hi;
-          }
-          wg_fence();
-#pragma unroll
-          for (int s = 0; s < H / 8; ++s) {
-            const uint32_t h0 = __float_as_uint(d0[h][4 * s]), h1 = __float_as_uint(d0[h][4 * s + 2]),
-                           h2 = __float_as_uint(d0[h][4 * s + 1]), h3 = __float_as_uint(d0[h][4 * s + 3]);
-            wg_mma_n64_rs(d1, lo[4 * s], lo[4 * s + 2], lo[4 * s + 1], lo[4 * s + 3], w1h_d + s * W_STEP, s > 0);
-            wg_mma_n64_rs(d1, h0, h1, h2, h3, w1l_d + s * W_STEP, 1);
-            wg_mma_n64_rs(d1, h0, h1, h2, h3, w1h_d + s * W_STEP, 1);
-          }
-          wg_commit();
-          wg_wait0();
-          clk.lap(2);
-          // ---- last hidden layer: bias, gate, output head(s), results
-          gate(d1, s_b1);
-          head(d1, o);
-          store(T, h, o);
+        for (int e = 0; e < 32; ++e) {
+          const float hi = __uint_as_float(__float_as_uint(d0[e]) & TF32_MASK);
+          lo[e] = __float_as_uint(d0[e] - hi);
+          d0[e] = hi;
         }
+        wg_fence();
+        ws_unroll<H / 8>([&](auto S) {
+          constexpr int s = decltype(S)::value, WO = s * W_STEP;
+          const uint32_t h0 = __float_as_uint(d0[4 * s]), h1 = __float_as_uint(d0[4 * s + 2]), h2 = __float_as_uint(d0[4 * s + 1]),
+                         h3 = __float_as_uint(d0[4 * s + 3]);
+          wg_mma_n64_rs_at<WO>(d1, lo[4 * s], lo[4 * s + 2], lo[4 * s + 1], lo[4 * s + 3], w1h_d, s > 0);
+          wg_mma_n64_rs_at<WO>(d1, h0, h1, h2, h3, w1l_d, 1);
+          wg_mma_n64_rs_at<WO>(d1, h0, h1, h2, h3, w1h_d, 1);
+        });
+        wg_commit();
+        wg_wait0();
+        clk.lap(2);
+        // ---- last hidden layer: bias, gate, output head(s), results
+        gate(d1, s_b1);
+        head(d1, o);
+        store(T, o);
       } else {
         // single hidden layer: its bias came through the MMA
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          gate(d0[h], nullptr);
-          head(d0[h], o);
-          store(T, h, o);
-        }
+        gate(d0, nullptr);
+        head(d0, o);
+        store(T, o);
       }
       clk.lap(3);
     }
-  } else if (warp < WS_CW + WS_GT * WS_GW) {
+  } else {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(WS_REG_G));
     // =====================================================================================================
     // G: gather teams -- the 4 warps of a team work on the same tile, each on its share of the queries: per round a
     // lane has GU passes x K feature-row loads (16 x LDG.128 for F = 32) in flight; the two teams (and the ring of A
     // tiles) overlap one team's load latency with the other team's reduction.  (A register double buffer over the
     // passes of ONE warp was tried: it spills inside the loop at 120 registers and lost 5 %.)
+    //
+    // The teams also fill the meta ring: TMA bulk copies (cp.async.bulk, completion counted in bytes on the block's
+    // "full" mbarrier; no thread touches the data) of what search_kernel wrote for a 32-query block -- neighbour ids +
+    // IDW weights (2 KB), position part (384 B) and, with d/dq, the forward-mode seeds (4.1 KB).  Block blk + MB of the
+    // ring belongs to the same team as block blk, so a team refills its own slots: position j of the team's stream of
+    // meta blocks takes the slot of position j - MD, and before it works on position j one warp of the team (in
+    // turn) issues position j + PF, whose slot the team left two positions ago.
     // profile slots: 0 wait free A tile, 1 wait meta block, 2 feature-row loads issued, 3 reduce + A-tile stores,
-    //                4 position rows + fence + arrive
+    //                4 position rows + fence + arrive, 5 meta refill (wait free slot + copies), 6 wait for the search grid
     // =====================================================================================================
     const int team = (warp - WS_CW) / WS_GW, gw = (warp - WS_CW) % WS_GW;
     const int sub = lane / M::LPR, c4 = lane % M::LPR;
     const float4* __restrict__ f4 = reinterpret_cast<const float4*>(p.feat) + c4;
     constexpr int GU = NPASS / WS_GW >= 2 ? 2 : 1;  // passes in flight per gather warp
-    int i = team;
+    static_assert(MB % (WS_GT * BPT) == 0, "the slots of a team's meta blocks repeat every MB blocks");
+    constexpr int MD = MB / WS_GT;  // meta slots per team
+    constexpr int PF = MD - 2;      // meta blocks in flight ahead of the one being gathered
+    static_assert(PF >= 1, "meta ring too small to refill ahead");
+    // position jj of this team's stream: block b = jj % BPT of its tile i = team + WS_GT * (jj / BPT)
+    auto refill = [&](int jj) {
+      if (jj % WS_GW != gw) return;
+      const int ri = team + WS_GT * (jj / BPT), b = jj % BPT;
+      const long long T = blockIdx.x + (long long)ri * gridDim.x;
+      if (T >= n_tiles) return;
+      const int blk = ri * BPT + b, ms = blk % MB;
+      ws_wait_relaxed(um_smem_u32(bars + WSB_META_EMPTY + ms), ((uint32_t)(blk / MB) & 1u) ^ 1u);
+      float* mt = meta + ms * MSTRIDE;
+      const uint32_t full = um_smem_u32(bars + WSB_META_FULL + ms);
+      const long long st = T * BPT + b;  // stash block
+      if (st < n_blocks) {
+        if (ws_elect()) {
+          const float* sb = p.stash + (size_t)st * Stash::floats;
+          constexpr uint32_t B_LW = 2 * WT * 8 * 4, B_XN = 3 * WT * 4, B_SD = Seeds::floats * 4;
+          ws_arrive_expect_tx(full, B_LW + B_XN + (GRAD ? B_SD : 0u));
+          ws_bulk_g2s(mt + WsMeta::li, sb + Stash::li, B_LW, full);  // li | w are adjacent in both layouts
+          ws_bulk_g2s(mt + WsMeta::xn, sb + Stash::pos, B_XN, full);
+          if (GRAD) ws_bulk_g2s(mt + WsMeta::om, p.seeds + (size_t)st * Seeds::floats, B_SD, full);
+        }
+      } else {  // tail of the last value-only tile: a block without neighbours
+        for (int e = lane; e < MSTRIDE; e += 32) mt[e] = e < WsMeta::w ? __int_as_float(-1) : 0.f;
+        __syncwarp();
+        if (lane == 0) ws_arrive(full);
+      }
+      __syncwarp();
+    };
+    // the meta copies read what the search launch wrote: with programmatic dependent launch this grid may have
+    // started before that one finished
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    clk.lap(6);
+    for (int jj = 0; jj < PF; ++jj) refill(jj);
+    clk.lap(5);
+    int i = team, j = 0;
     for (long long T = blockIdx.x + (long long)team * gridDim.x; T < n_tiles; T += (long long)WS_GT * gridDim.x, i += WS_GT) {
       const int slot = i % WS_A0;
       unsigned char* a_hi = sm + lay.a0 + slot * lay.a0_stride;
       unsigned char* a_lo = a_hi + lay.a0_half;
       bool slot_free = false;
 #pragma unroll 1
-      for (int b = 0; b < BPT; ++b) {
+      for (int b = 0; b < BPT; ++b, ++j) {
+        refill(j + PF);
+        clk.lap(5);
         const int blk = i * BPT + b, ms = blk % MB;
         ws_wait_relaxed(um_smem_u32(bars + WSB_META_FULL + ms), (uint32_t)(blk / MB) & 1u);
         clk.lap(1);
@@ -520,50 +577,8 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       }
       if (lane == 0) ws_arrive(um_smem_u32(bars + WSB_A0_FULL + slot));
     }
-  } else {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(WS_REG_L));
-    // =====================================================================================================
-    // L: loader warps -- TMA bulk copies of the search launch's results into the meta ring: neighbour ids + IDW weights
-    // (2 KB), position part (384 B) and, with d/dq, the forward-mode seeds (4.1 KB) of a 32-query block, all counted in
-    // bytes on the block's "full" mbarrier.  No thread touches the data.
-    // profile slots: 0 wait free meta block, 1 copies issued
-    // =====================================================================================================
-    const int lw = warp - WS_CW - WS_GT * WS_GW;
-    // the only role that reads what the search launch wrote: with programmatic dependent launch this grid may have
-    // started before that one finished
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    int i = 0;
-    for (long long T = blockIdx.x; T < n_tiles; T += gridDim.x, ++i) {
-#pragma unroll 1
-      for (int b = 0; b < BPT; ++b) {
-        const int blk = i * BPT + b;
-        if (blk % WS_LW != lw) continue;
-        const int ms = blk % MB;
-        ws_wait_relaxed(um_smem_u32(bars + WSB_META_EMPTY + ms), ((uint32_t)(blk / MB) & 1u) ^ 1u);
-        clk.lap(0);
-        float* mt = meta + ms * MSTRIDE;
-        const uint32_t full = um_smem_u32(bars + WSB_META_FULL + ms);
-        const long long st = T * BPT + b;  // stash block
-        if (st < n_blocks) {
-          if (ws_elect()) {
-            const float* sb = p.stash + (size_t)st * Stash::floats;
-            constexpr uint32_t B_LW = 2 * WT * 8 * 4, B_XN = 3 * WT * 4, B_SD = Seeds::floats * 4;
-            ws_arrive_expect_tx(full, B_LW + B_XN + (GRAD ? B_SD : 0u));
-            ws_bulk_g2s(mt + WsMeta::li, sb + Stash::li, B_LW, full);  // li | w are adjacent in both layouts
-            ws_bulk_g2s(mt + WsMeta::xn, sb + Stash::pos, B_XN, full);
-            if (GRAD) ws_bulk_g2s(mt + WsMeta::om, p.seeds + (size_t)st * Seeds::floats, B_SD, full);
-          }
-        } else {  // tail of the last value-only tile: a block without neighbours
-          for (int e = lane; e < MSTRIDE; e += 32) mt[e] = e < WsMeta::w ? __int_as_float(-1) : 0.f;
-          __syncwarp();
-          if (lane == 0) ws_arrive(full);
-        }
-        __syncwarp();
-        clk.lap(1);
-      }
-    }
   }
-  clk.flush(warp);
+  clk.flush(warp, warp < WS_CW ? WS_ROLE_C : WS_ROLE_G);
 }
 
 // ---------------------------------------------------------------------------

@@ -1,14 +1,31 @@
-"""A/B of the two decode variants of the split pipeline at BASELINE cfg2 (200k queries): python scripts/exp_decode.py"""
+"""Where the time of K1 (search launch + decode launch) goes at BASELINE cfg2 (200k queries, K = 8, F = 32, 2 x 64
+decoder, d sdf / dq), the headline workload of bench.py:
+
+  1. A/B of the two decode variants of the split pipeline (CUDA events, L2 flushed before every step)
+  2. per-kernel device time per step of the default variant (torch.profiler with CUDA activities, a run of its own);
+     with --out DIR the trace goes to DIR/exp_decode_trace.json
+  3. per-role cycle table of wsq_decode_kernel: per warp, clock deltas of the phases of its role, summed over one
+     profiled launch (ws_profile); the role of every warp is read from the counters, so the table follows the kernel
+
+python scripts/exp_decode.py [variant ...] [--steps N] [--out DIR]"""
+import argparse
 import os
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import numpy as np
 import torch
 
-from pin_slam_b200 import ops
+from pin_slam_b200 import _lib, ops
 from pin_slam_b200.config import HotPathConfig
 from pin_slam_b200.model import Decoder
 from pin_slam_b200.synthetic import build_map, surface_queries
+
+ap = argparse.ArgumentParser()
+ap.add_argument("variants", type=int, nargs="*", default=[0, 1])
+ap.add_argument("--steps", type=int, default=20, help="steps of the profiled run")
+ap.add_argument("--out", default=None, help="directory for the profiler trace")
+args = ap.parse_args()
 
 dev = torch.device("cuda:0")
 flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
@@ -34,7 +51,8 @@ def timed(fn, n=10):
     return ts[len(ts) // 2], ts[0]
 
 
-for variant in [int(a) for a in sys.argv[1:]] or [0, 1]:
+# ---- 1. decode variants
+for variant in args.variants:
     ops.set_option("decode_variant", variant)
     out = {}
     ts = []
@@ -59,21 +77,70 @@ for variant in [int(a) for a in sys.argv[1:]] or [0, 1]:
     med, mn = timed(lambda: npm.query_sdf(q, dec, need_grad=False, out=o2))
     print(f"variant {variant}: value-only (need_grad=False) cold-L2 median {med:.4f} ms, min {mn:.4f} ms", flush=True)
 
-# per-warp phase cycle counters of the warp-specialised decode (one profiled launch)
-import numpy as np
-from pin_slam_b200 import _lib
+# ---- 2. per-kernel device time of the warp-specialised decode variant (the default)
+from torch.profiler import ProfilerActivity, profile
+
 ops.set_option("decode_variant", 1)
+out = {}
+for _ in range(3):
+    npm.query_sdf(q, dec, out=out)
+torch.cuda.synchronize()
+with profile(activities=[ProfilerActivity.CUDA]) as tp:
+    for _ in range(args.steps):
+        flush.zero_()
+        npm.query_sdf(q, dec, out=out)
+    torch.cuda.synchronize()
+if args.out:
+    os.makedirs(args.out, exist_ok=True)
+    tp.export_chrome_trace(os.path.join(args.out, "exp_decode_trace.json"))
+rows = []
+for e in tp.key_averages():
+    t = getattr(e, "device_time_total", None)
+    if t is None:
+        t = e.cuda_time_total
+    if t > 0:
+        rows.append((t / args.steps, e.count / args.steps, e.key))
+print(f"device time per step over {args.steps} profiled steps (flush = the L2 flush between steps, not part of K1):")
+k1 = 0.0
+for t, n, name in sorted(rows, reverse=True):
+    tag = "flush" if "search_kernel" not in name and "wsq_decode_kernel" not in name else "K1"
+    if tag == "K1":
+        k1 += t
+    print(f"  {t:9.1f} us  {n:5.2f} launches  [{tag:5s}] {name[:110]}")
+print(f"  {k1:9.1f} us  K1 kernels per step (sum)", flush=True)
+
+# ---- 3. per-role cycle table of one profiled launch of wsq_decode_kernel<32, true, true>
+# role codes as written by wsq.cu (WS_ROLE_*) -> (name, slot names, indices of the slots that are waits)
+ROLES = {
+    1: ("C consumer", ["wait_A", "layer0", "layer1", "last+out"], {0}),
+    2: ("G gather", ["wait_A_free", "wait_meta", "issue_loads", "reduce+store", "pos+fence"], {0, 1}),
+    3: ("L loader", ["wait_meta_free", "copies"], {0}),
+    4: ("G gather + meta refill", ["wait_A_free", "wait_meta", "issue_loads", "reduce+store", "pos+fence",
+                                   "meta_refill", "wait_search"], {0, 1, 6}),
+}
+N_CTA, N_WARP, N_SLOT = 132, 16, 8
 ops.set_option("ws_profile", 1)
 npm.query_sdf(q, dec, out=out)
 torch.cuda.synchronize()
 ops.set_option("ws_profile", 0)
-buf = np.zeros(132 * 16 * 8, dtype=np.uint64)
+buf = np.zeros(N_CTA * N_WARP * N_SLOT, dtype=np.uint64)
 _lib.check(_lib.load().pinb200_debug_read(b"ws_profile", buf.ctypes.data, buf.size), "debug_read")
-prof = buf.reshape(132, 16, 8).astype(np.float64)
-names = {"E": ["wait_mma0", "epi0", "-", "wait_mma1", "epi1", "outputs"], "M": ["wait_A1", "wait_D1free", "issue_L1", "wait_Atile", "issue_L0"], "G": ["wait_A_free", "wait_meta", "issue_loads", "reduce+store", "pos+fence"],
-         "L": ["wait_meta_free", "stash_loads", "seeds+store"]}
-for role, ws in (("E", range(0, 8)), ("G", range(8, 16)), ("L", range(16, 18)), ("M", range(18, 20))):
-    med = np.median(prof[:, list(ws), :], axis=0)  # [warps, slots] median over CTAs
-    print(role, "median cycles per warp over the launch (", ", ".join(names[role]), "):")
-    for w, row in zip(ws, med):
-        print(f"  warp {w:2d}: " + "  ".join(f"{int(v):8d}" for v in row[:len(names[role])]) + f"   total {int(row.sum()):8d}")
+prof = buf.reshape(N_CTA, N_WARP, N_SLOT)
+ran = prof[:, :, N_SLOT - 1].max(axis=1) > 0  # CTAs of the launch (grid <= SM count)
+role_of = prof[ran][0, :, N_SLOT - 1].astype(int)
+cyc = prof[ran][:, :, : N_SLOT - 1].astype(np.float64)
+med = np.median(cyc, axis=0)  # [warp, slot] median over CTAs
+launch = med.sum(axis=1).max()
+print(f"wsq_decode_kernel per-warp cycles, median over {int(ran.sum())} CTAs; longest warp {int(launch)} cycles")
+for code in sorted(set(role_of.tolist())):
+    name, slots, waits = ROLES[code]
+    ws = [w for w in range(N_WARP) if role_of[w] == code]
+    print(f"{name}: warps {ws[0]}-{ws[-1]}  ({', '.join(slots)})")
+    for w in ws:
+        row = med[w, : len(slots)]
+        print(f"  warp {w:2d}: " + "  ".join(f"{int(v):9d}" for v in row) + f"   total {int(row.sum()):9d}")
+    tot = med[ws, : len(slots)].sum(axis=0)
+    share = tot / tot.sum()
+    busy = 1.0 - sum(share[s] for s in waits)
+    print("  share:   " + "  ".join(f"{100 * s:8.1f}%" for s in share) +
+          f"   busy (not waiting on another role) {100 * busy:.1f}%", flush=True)

@@ -26,8 +26,9 @@ namespace pinb {
 
 // K1a of the split pipeline: phase A1 alone, at high occupancy (no decoder weights in shared memory, <= 128
 // registers): the probe rounds of ~16 resident warps per SM keep the load/store unit busy, which the fused kernel's
-// 12 warps (most of them in compute phases at any time) cannot.  One warp = one 32-query tile.
-template <bool SEEDS>
+// 12 warps (most of them in compute phases at any time) cannot.  One warp = one 32-query tile.  SORTED: the tiles
+// are runs of p.perm (spatially sorted queries), and the stash blocks are StashS blocks.
+template <bool SEEDS, bool SORTED>
 __global__ void __launch_bounds__(128, 4) search_kernel(const __grid_constant__ QueryParams p) {
   extern __shared__ __align__(16) float smem[];
   uint32_t* s_delta = reinterpret_cast<uint32_t*>(smem);
@@ -38,7 +39,8 @@ __global__ void __launch_bounds__(128, 4) search_kernel(const __grid_constant__ 
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
   for (int st = blockIdx.x * nwarp + warp; st < p.n_tiles; st += gridDim.x * nwarp)
-    a1_tile<SEEDS>(p, s_delta, (long long)st * WT, WT, lane, p.stash + (size_t)st * Stash::floats);
+    a1_tile<SEEDS, SORTED>(p, s_delta, (long long)st * WT, WT, lane,
+                           p.stash + (size_t)st * (SORTED ? StashS::floats : Stash::floats));
 }
 
 // ---------------------------------------------------------------------------
@@ -489,6 +491,8 @@ namespace pinb {
 static long long g_split_min_queries = PINB200_SPLIT_MIN_QUERIES;        // decode-every-neighbour maps (mma.sync decode)
 static long long g_split_min_queries_wf = PINB200_SPLIT_MIN_QUERIES_WF;  // weighted_first maps (tensor-core decode)
 static int g_decode_variant = 1;  // 0: decode_umma_kernel (phase-synchronous, backward MMAs), 1: wsq_decode_kernel
+static long long g_sort_min_queries = PINB200_SORT_MIN_QUERIES;  // spatial sort before the search launch; 0: never
+static long long g_sort_min_queries_color = 0;                    // the same for calls with a colour head
 
 // ---------------------------------------------------------------------------
 // host side
@@ -634,10 +638,18 @@ static int launch_search(QueryParams& p, cudaStream_t stream) {
   p.n_tiles = (int)((p.n + WT - 1) / WT);
   const long long ctas = (p.n_tiles + 3) / 4;
   const int grid = (int)std::min<long long>(ctas, (long long)sm_count() * 4);
-  if (p.seeds)
-    search_kernel<true><<<grid, 128, align4(p.map.n_probe) * sizeof(float), stream>>>(p);
-  else
-    search_kernel<false><<<grid, 128, align4(p.map.n_probe) * sizeof(float), stream>>>(p);
+  const size_t smem = align4(p.map.n_probe) * sizeof(float);
+  if (p.perm) {
+    if (p.seeds)
+      search_kernel<true, true><<<grid, 128, smem, stream>>>(p);
+    else
+      search_kernel<false, true><<<grid, 128, smem, stream>>>(p);
+  } else {
+    if (p.seeds)
+      search_kernel<true, false><<<grid, 128, smem, stream>>>(p);
+    else
+      search_kernel<false, false><<<grid, 128, smem, stream>>>(p);
+  }
   return check_launch("search_kernel");
 }
 
@@ -723,7 +735,27 @@ extern "C" int pinb200_query_sdf(const pinb200_map_view* map, const pinb200_deco
     // the warp-specialised decode takes the forward-mode seeds of d/dq from the search launch (second workspace region)
     const bool want_seeds = g_decode_variant == 1 && umma_decode_supported(p) &&
                             (opts->need_grad || (color_dec && opts->need_grad && out->color_grad));
-    p.seeds = want_seeds ? p.stash + (size_t)p.n_tiles * Stash::floats : nullptr;
+    // Large inference batches whose decodes all run on wsq_decode_kernel are searched in Morton order of their cells
+    // (2x the map resolution): the lanes of a tile then probe the same or neighbouring cells.  Their stash blocks are
+    // compact (StashS), which leaves room in the workspace for the sort (query_sort.cu); if it does not fit, the batch
+    // runs unsorted.  Calls with a colour head have their own threshold, off by default: the large one (the dense
+    // RGB-D query) comes in pixel order, already coherent, and sorting it only adds the sort (0.420 -> 0.487 ms at
+    // 307 k pixels, H100 at 400 W).
+    const long long sort_min = color_dec ? g_sort_min_queries_color : g_sort_min_queries;
+    bool sorted = false;
+    if (sort_min > 0 && n >= sort_min && g_decode_variant == 1 && !opts->training_mode && umma_decode_supported(p)) {
+      QueryParams c = p;
+      if (color_dec) c.dec = *color_dec;
+      if (umma_decode_supported(c)) {
+        char* base = static_cast<char*>(opts->workspace);
+        const size_t used = (size_t)p.n_tiles * (StashS::floats + (want_seeds ? Seeds::floats : 0)) * sizeof(float);
+        rc = sort_queries(query_xyz, opts->transform, n, map->resolution, base + used,
+                          (size_t)opts->workspace_bytes - used, &p.perm, (cudaStream_t)stream);
+        if (rc) return rc;
+        sorted = p.perm != nullptr;
+      }
+    }
+    p.seeds = want_seeds ? p.stash + (size_t)p.n_tiles * (sorted ? StashS::floats : Stash::floats) : nullptr;
     rc = launch_search(p, (cudaStream_t)stream);
     if (rc) return rc;
   }
@@ -773,6 +805,18 @@ extern "C" int pinb200_set_option(const char* name, int64_t value) {
       return PINB200_ERR_BAD_ARG;
     }
     g_decode_variant = (int)value;
+  } else if (key == "sort_min_queries") {  // batches of at least this many queries are sorted; 0: never
+    if (value < 0) {
+      set_error("set_option: sort_min_queries %lld < 0", (long long)value);
+      return PINB200_ERR_BAD_ARG;
+    }
+    g_sort_min_queries = value;
+  } else if (key == "sort_min_queries_color") {  // the same for calls with a colour head; 0 (default): never
+    if (value < 0) {
+      set_error("set_option: sort_min_queries_color %lld < 0", (long long)value);
+      return PINB200_ERR_BAD_ARG;
+    }
+    g_sort_min_queries_color = value;
   } else if (key == "ws_profile") {
     wsq_set_profile(value != 0);
   } else {

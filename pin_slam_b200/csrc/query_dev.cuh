@@ -51,6 +51,10 @@ struct QueryParams {
   float* seeds;  // split pipeline with d/dq on the warp-specialised decode: [n_tiles][Seeds::floats] forward-mode seeds
   int pdl;       // host only: this decode launch directly follows its search launch (programmatic dependent launch)
   QueryLayout lay;
+  // split pipeline with spatially sorted queries: perm[i] = original index of the i-th query in sorted order (the
+  // search launch then works on perm[32 st + lane] and writes the compact StashS blocks; the decode stores row
+  // results at the original index).  nullptr: queries in the caller's order, Stash blocks.
+  const int32_t* perm;
 };
 
 // squared distance with the reference's arithmetic: sum((p - q)^2) in fp32, no contraction (:990-994)
@@ -346,6 +350,17 @@ struct Stash {
   static constexpr int floats = pos + WT * 3;
 };
 static_assert(Stash::floats % 4 == 0, "stash block is copied with 16-byte accesses");
+// The block of a sorted launch (QueryParams::perm) holds only what the warp-specialised decode reads, in the order of
+// the decode's meta block (one bulk copy): neighbour ids, IDW weights, position part, and the original index of every
+// query of the tile (-1 past the end of the batch).
+struct StashS {
+  static constexpr int li = 0;
+  static constexpr int w = li + WT * 8;
+  static constexpr int pos = w + WT * 8;
+  static constexpr int perm = pos + WT * 3;
+  static constexpr int floats = perm + WT;
+};
+static_assert(StashS::li == Stash::li && StashS::w == Stash::w && StashS::floats % 4 == 0, "li | w lead both layouts");
 
 // Forward-mode seeds of d sdf / d q for one query (wsq.cu pushes them through the decoder as tangent rows):
 //   w_k = u_k / sum u,  u_k = 1 / (d_k^2 + eps)  =>  omega_kj = d w_k / d q_j = w_k (c_k d_kj - sum_m w_m c_m d_mj),
@@ -432,7 +447,9 @@ __device__ __forceinline__ void tangent_seeds(const pinb200_map_view& m, int K, 
     for (int i = 0; i < 3; ++i) sd[Seeds::P + (j * 3 + i) * WT + lane] = P[j][i];
 }
 
-template <bool SEEDS = false>
+// SORTED: lane `lane` works on query p.perm[q0s + lane] (per-query outputs go to that index) and `stash` is a StashS
+// block; the seeds stay in tile order.
+template <bool SEEDS = false, bool SORTED = false>
 __device__ __forceinline__ void a1_tile(const QueryParams& p, const uint32_t* s_delta, long long q0s, int WQ, int lane,
                                         float* stash) {
   const pinb200_map_view& m = p.map;
@@ -445,9 +462,13 @@ __device__ __forceinline__ void a1_tile(const QueryParams& p, const uint32_t* s_
   float* s_q = stash + Stash::q;
   float* s_usum = stash + Stash::usum;
   int* s_nn = reinterpret_cast<int*>(stash + Stash::nn);
-  float* s_pos = stash + Stash::pos;
-  const long long qi = q0s + lane;
-  const bool live = lane < WQ && qi < p.n;
+  float* s_pos = stash + (SORTED ? StashS::pos : Stash::pos);
+  const bool live = lane < WQ && q0s + lane < p.n;
+  long long qi = q0s + lane;
+  if (SORTED) {
+    qi = live ? (long long)__ldg(p.perm + q0s + lane) : -1;
+    reinterpret_cast<int*>(stash + StashS::perm)[lane] = (int)qi;
+  }
   float qx = 0.f, qy = 0.f, qz = 0.f;
   if (live) {
     qx = __ldg(p.query_xyz + 3 * qi + 0);
@@ -551,16 +572,20 @@ __device__ __forceinline__ void a1_tile(const QueryParams& p, const uint32_t* s_
     if (k < K) {
       s_li[k * WT + lane] = lif[k];
       s_w[k * WT + lane] = w[k];
-      s_dx[k * WT + lane] = dx;
-      s_dy[k * WT + lane] = dy;
-      s_dz[k * WT + lane] = dz;
+      if (!SORTED) {
+        s_dx[k * WT + lane] = dx;
+        s_dy[k * WT + lane] = dy;
+        s_dz[k * WT + lane] = dz;
+      }
     }
   }
-  s_nn[lane] = cnt;
-  s_usum[lane] = usum;
-  s_q[0 * WT + lane] = qx;
-  s_q[1 * WT + lane] = qy;
-  s_q[2 * WT + lane] = qz;
+  if (!SORTED) {
+    s_nn[lane] = cnt;
+    s_usum[lane] = usum;
+    s_q[0 * WT + lane] = qx;
+    s_q[1 * WT + lane] = qy;
+    s_q[2 * WT + lane] = qz;
+  }
   s_pos[0 * WT + lane] = sx;  // position part of the IDW-averaged decoder input (weighted_first)
   s_pos[1 * WT + lane] = sy;
   s_pos[2 * WT + lane] = sz;
@@ -601,5 +626,7 @@ struct QueryParams;
 int dispatch_wsq(QueryParams& p, cudaStream_t stream);  // wsq.cu
 void wsq_set_profile(int on);
 int wsq_read_profile(unsigned long long* host_out, int64_t count);
+int sort_queries(const float* xyz, const double* transform, long long n, float resolution, void* scratch,
+                 size_t scratch_bytes, const int32_t** perm, cudaStream_t stream);  // query_sort.cu
 
 }  // namespace pinb

@@ -41,12 +41,17 @@ constexpr int WS_THREADS = (WS_CW + WS_GT * WS_GW) * 32;
 constexpr int WS_REG_C = 136, WS_REG_G = 120;
 static_assert((WS_CW * WS_REG_C + WS_GT * WS_GW * WS_REG_G) * 32 <= WS_THREADS * 128, "setmaxnreg pool");
 constexpr int WS_A0 = 2;       // A-tile ring slots, one per gather team
+// ring of the original query indices of a tile (sorted launches): tile i in slot i % WS_QX.  Slot i % WS_QX is
+// rewritten for tile i + WS_QX only after the A tile of tile i + WS_A0 was released, i.e. after every consumer warp
+// stored tile i
+constexpr int WS_QX = 2 * WS_A0;
 
 struct WsMeta {  // float offsets inside a meta block of 32 queries, [field][k][lane]
   static constexpr int li = 0;                   // [8][32] neighbour id | REMAP, -1 invalid
   static constexpr int w = li + WT * 8;          // [8][32] IDW weight
   static constexpr int xn = w + WT * 8;          // [3][32] sum_k w_k n_k
-  static constexpr int floats_ng = xn + WT * 3;
+  static constexpr int perm = xn + WT * 3;       // [32] original query index (sorted launches only)
+  static constexpr int floats_ng = perm + WT;
   static constexpr int om = floats_ng;           // [3][8][32] d w_k / d q_j
   static constexpr int P = om + WT * 24;         // [3 j][3 i][32] d (sum_k w_k n_k)_i / d q_j
   static constexpr int floats_g = P + WT * 9;
@@ -55,6 +60,7 @@ struct WsMeta {  // float offsets inside a meta block of 32 queries, [field][k][
 struct WsLayout {  // byte offsets from the dynamic shared memory base
   int w0_hi, w0_lo, w1_hi, w1_lo, b0, b1, wout, bout;
   int a0, a0_half, a0_stride;  // ring of A tiles: slot s = [a0 + s*stride: hi | + half: lo]
+  int qidx;                    // [WS_QX][128] original query index of every tile row's query (sorted launches)
   int meta, meta_stride, n_meta;
   int bars, total;
 };
@@ -144,6 +150,8 @@ __device__ __forceinline__ void ws_arrive(uint32_t bar) {
 
 static_assert(WsMeta::P - WsMeta::om == Seeds::P - Seeds::om && WsMeta::floats_g - WsMeta::om == Seeds::floats,
               "the seed block of the search launch is copied verbatim into the meta block");
+static_assert(WsMeta::xn == StashS::pos && WsMeta::perm == StashS::perm && WsMeta::floats_ng == StashS::floats,
+              "a sorted launch's stash block is the head of the meta block (one bulk copy)");
 
 // fn(std::integral_constant<int, s>) for s = 0 .. N-1: a k-step loop whose step is a compile-time constant
 template <typename Fn, int... S>
@@ -312,8 +320,11 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       out_qstride = p.is_color ? 3 * OC : 3;
       out_chstride = 3;
     }
-    // value rows write the prediction, tangent rows one component of its gradient; lane c == r of the quad writes row r
-    auto store = [&](long long T, float (&o)[2][4]) {
+    // value rows write the prediction, tangent rows one component of its gradient; lane c == r of the quad writes row r.
+    // Tile i holds queries T * QT .. in search order; a sorted launch maps them to their original index through the
+    // index ring the gather team filled (shared memory: no global load on this path)
+    const int* s_qidx = reinterpret_cast<const int*>(sm + lay.qidx);
+    auto store = [&](long long T, int i, float (&o)[2][4]) {
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         if (p.dec.sigmoid_out) {
@@ -330,9 +341,10 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
 #pragma unroll
           for (int ch = 0; ch < 4; ++ch) o[r][ch] = fmaf(bsel, s_bout[ch], o[r][ch]) * p.dec.out_scale;
         }
-        const int row = 64 * h + 16 * wq + g8 + 8 * r;
-        const long long qi = T * QT + (GRAD ? (row >> 2) : row);
+        const int row = 64 * h + 16 * wq + g8 + 8 * r, qrow = GRAD ? (row >> 2) : row;
+        long long qi = T * QT + qrow;
         if (c == r && qi < p.n) {
+          if (p.perm) qi = s_qidx[(i % WS_QX) * QT + qrow];
           if (out_base) {
             float* dst = out_base + qi * out_qstride;
 #pragma unroll
@@ -399,12 +411,12 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
         // ---- last hidden layer: bias, gate, output head(s), results
         gate(d1, s_b1);
         head(d1, o);
-        store(T, o);
+        store(T, i, o);
       } else {
         // single hidden layer: its bias came through the MMA
         gate(d0, nullptr);
         head(d0, o);
-        store(T, o);
+        store(T, i, o);
       }
       clk.lap(3);
     }
@@ -446,11 +458,16 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       const long long st = T * BPT + b;  // stash block
       if (st < n_blocks) {
         if (ws_elect()) {
-          const float* sb = p.stash + (size_t)st * Stash::floats;
-          constexpr uint32_t B_LW = 2 * WT * 8 * 4, B_XN = 3 * WT * 4, B_SD = Seeds::floats * 4;
-          ws_arrive_expect_tx(full, B_LW + B_XN + (GRAD ? B_SD : 0u));
-          ws_bulk_g2s(mt + WsMeta::li, sb + Stash::li, B_LW, full);  // li | w are adjacent in both layouts
-          ws_bulk_g2s(mt + WsMeta::xn, sb + Stash::pos, B_XN, full);
+          constexpr uint32_t B_LW = 2 * WT * 8 * 4, B_XN = 3 * WT * 4, B_S = StashS::floats * 4, B_SD = Seeds::floats * 4;
+          if (p.perm) {  // li | w | pos | perm: one copy
+            ws_arrive_expect_tx(full, B_S + (GRAD ? B_SD : 0u));
+            ws_bulk_g2s(mt, p.stash + (size_t)st * StashS::floats, B_S, full);
+          } else {
+            const float* sb = p.stash + (size_t)st * Stash::floats;
+            ws_arrive_expect_tx(full, B_LW + B_XN + (GRAD ? B_SD : 0u));
+            ws_bulk_g2s(mt + WsMeta::li, sb + Stash::li, B_LW, full);  // li | w are adjacent in both layouts
+            ws_bulk_g2s(mt + WsMeta::xn, sb + Stash::pos, B_XN, full);
+          }
           if (GRAD) ws_bulk_g2s(mt + WsMeta::om, p.seeds + (size_t)st * Seeds::floats, B_SD, full);
         }
       } else {  // tail of the last value-only tile: a block without neighbours
@@ -553,6 +570,9 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
           ws_wait_relaxed(um_smem_u32(bars + WSB_A0_EMPTY + slot), ((uint32_t)(i / WS_A0) & 1u) ^ 1u);
           slot_free = true;
         }
+        // the tile's original query indices, for the consumers' stores (the meta slot is refilled before they store)
+        if (p.perm && (b % WS_GW) == gw)
+          reinterpret_cast<int*>(sm + lay.qidx)[(i % WS_QX) * QT + b * WT + lane] = reinterpret_cast<const int*>(mt + WsMeta::perm)[lane];
         // position part (columns F .. F+2) and zero padding of the rows: thread per row
         if (GRAD || (b % WS_GW) == gw) {
           const int row = GRAD ? gw * WT + lane : b * WT + lane;
@@ -608,6 +628,7 @@ static WsLayout plan_ws_layout(const pinb200_decoder_view& d, bool grad) {
   l.a0_half = ((UM_ROWS / 8) * (DM::K0 / 4) * UM_A_LBO + 127) & ~127;
   l.a0_stride = 2 * l.a0_half;
   l.a0 = take(WS_A0 * l.a0_stride);
+  l.qidx = take(WS_QX * 128 * 4);
   l.meta_stride = (grad ? WsMeta::floats_g : WsMeta::floats_ng) * 4;
   l.n_meta = grad ? 8 : 16;
   l.meta = take(l.n_meta * l.meta_stride);

@@ -10,6 +10,7 @@ from ._lib import DecoderView, GnOpts, MapTrainOpts, MapView, QueryOpts, QueryOu
 
 SPLIT_MIN_QUERIES = 32768  # == PINB200_SPLIT_MIN_QUERIES (default; see set_option)
 SPLIT_MIN_QUERIES_WF = 1024  # == PINB200_SPLIT_MIN_QUERIES_WF: weighted_first maps on the tensor-core decode
+SORT_MIN_QUERIES = 131072  # == PINB200_SORT_MIN_QUERIES: spatial sort before the search launch (see set_option)
 
 
 def uses_split(n: int, weighted_first: bool, dec=None, training_mode: bool = False) -> bool:
@@ -22,7 +23,8 @@ def uses_split(n: int, weighted_first: bool, dec=None, training_mode: bool = Fal
 
 
 def set_option(name: str, value: int) -> None:
-    """Process-wide tunables of the query path (pinb200_set_option): "split_min_queries", "decode_variant"."""
+    """Process-wide tunables of the query path (pinb200_set_option): "split_min_queries", "decode_variant",
+    "sort_min_queries" (0: never sort), "sort_min_queries_color" (calls with a colour head; default 0)."""
     global SPLIT_MIN_QUERIES, SPLIT_MIN_QUERIES_WF
     _lib.check(_lib.load().pinb200_set_option(name.encode(), int(value)), "pinb200_set_option")
     if name == "split_min_queries":

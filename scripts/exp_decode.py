@@ -7,7 +7,14 @@ decoder, d sdf / dq), the headline workload of bench.py:
   3. per-role cycle table of wsq_decode_kernel: per warp, clock deltas of the phases of its role, summed over one
      profiled launch (ws_profile); the role of every warp is read from the counters, so the table follows the kernel
 
-python scripts/exp_decode.py [variant ...] [--steps N] [--out DIR]"""
+Section 2 counts the launches of the in-library spatial sort (histogram memset, sort_key_kernel, the scan's kernels,
+sort_scatter_kernel) with K1.
+With --presorted it also runs with the sort off (sort_min_queries 0), on the bench's random queries and on the same
+queries pre-permuted in Python into Morton order of their 0.4 m cells: the best that sorting inside the library
+could reach, without its cost.  --sort-sweep times K1 with the sort off and on over batch sizes (CUDA events, L2
+flushed before every step), to place the default of sort_min_queries.
+
+python scripts/exp_decode.py [variant ...] [--steps N] [--out DIR] [--presorted] [--sort-sweep]"""
 import argparse
 import os
 import sys
@@ -25,6 +32,9 @@ ap = argparse.ArgumentParser()
 ap.add_argument("variants", type=int, nargs="*", default=[0, 1])
 ap.add_argument("--steps", type=int, default=20, help="steps of the profiled run")
 ap.add_argument("--out", default=None, help="directory for the profiler trace")
+ap.add_argument("--presorted", action="store_true",
+                help="also profile, with the sort off, the queries pre-permuted into Morton order of their cells")
+ap.add_argument("--sort-sweep", action="store_true", help="K1 time with the sort off / on over batch sizes")
 args = ap.parse_args()
 
 dev = torch.device("cuda:0")
@@ -80,34 +90,69 @@ for variant in args.variants:
 # ---- 2. per-kernel device time of the warp-specialised decode variant (the default)
 from torch.profiler import ProfilerActivity, profile
 
-ops.set_option("decode_variant", 1)
-out = {}
-for _ in range(3):
-    npm.query_sdf(q, dec, out=out)
-torch.cuda.synchronize()
-with profile(activities=[ProfilerActivity.CUDA]) as tp:
-    for _ in range(args.steps):
-        flush.zero_()
-        npm.query_sdf(q, dec, out=out)
+def morton_presort(x, cell=0.4):
+    """x[argsort(key)], key = 30-bit Morton interleave of floor(x / cell) (10 bits per axis, wrapped)."""
+    c = torch.floor(x / cell).long() & 1023
+    key = torch.zeros(x.shape[0], dtype=torch.long, device=x.device)
+    for b in range(10):
+        for a in range(3):
+            key |= ((c[:, a] >> b) & 1) << (3 * b + a)
+    return x[torch.argsort(key)].contiguous()
+
+
+def kernel_table(qq, label, trace_name):
+    out = {}
+    for _ in range(3):
+        npm.query_sdf(qq, dec, out=out)
     torch.cuda.synchronize()
-if args.out:
-    os.makedirs(args.out, exist_ok=True)
-    tp.export_chrome_trace(os.path.join(args.out, "exp_decode_trace.json"))
-rows = []
-for e in tp.key_averages():
-    t = getattr(e, "device_time_total", None)
-    if t is None:
-        t = e.cuda_time_total
-    if t > 0:
-        rows.append((t / args.steps, e.count / args.steps, e.key))
-print(f"device time per step over {args.steps} profiled steps (flush = the L2 flush between steps, not part of K1):")
-k1 = 0.0
-for t, n, name in sorted(rows, reverse=True):
-    tag = "flush" if "search_kernel" not in name and "wsq_decode_kernel" not in name else "K1"
-    if tag == "K1":
-        k1 += t
-    print(f"  {t:9.1f} us  {n:5.2f} launches  [{tag:5s}] {name[:110]}")
-print(f"  {k1:9.1f} us  K1 kernels per step (sum)", flush=True)
+    with profile(activities=[ProfilerActivity.CUDA]) as tp:
+        for _ in range(args.steps):
+            flush.zero_()
+            npm.query_sdf(qq, dec, out=out)
+        torch.cuda.synchronize()
+    if args.out:
+        os.makedirs(args.out, exist_ok=True)
+        tp.export_chrome_trace(os.path.join(args.out, trace_name))
+    rows = []
+    for e in tp.key_averages():
+        t = getattr(e, "device_time_total", None)
+        if t is None:
+            t = e.cuda_time_total
+        if t > 0:
+            rows.append((t / args.steps, e.count / args.steps, e.key))
+    print(f"{label}: device time per step over {args.steps} profiled steps (flush = the L2 flush between steps, "
+          "not part of K1):")
+    k1 = 0.0
+    for t, n, name in sorted(rows, reverse=True):
+        tag = "K1" if any(k in name for k in K1_KERNELS) else "flush"
+        if tag == "K1":
+            k1 += t
+        print(f"  {t:9.1f} us  {n:5.2f} launches  [{tag:5s}] {name[:110]}")
+    print(f"  {k1:9.1f} us  K1 kernels per step (sum)", flush=True)
+    return out
+
+
+K1_KERNELS = ("search_kernel", "wsq_decode_kernel", "sort_key_kernel", "DeviceScan", "sort_scatter_kernel", "Memset")
+ops.set_option("decode_variant", 1)
+out = kernel_table(q, "random queries, library defaults", "exp_decode_trace.json")
+if args.presorted:
+    ops.set_option("sort_min_queries", 0)
+    kernel_table(q, "random queries, sort off", "exp_decode_trace_unsorted.json")
+    kernel_table(morton_presort(q), "Morton-presorted queries, sort off", "exp_decode_trace_presorted.json")
+    ops.set_option("sort_min_queries", ops.SORT_MIN_QUERIES)
+if args.sort_sweep:
+    print("K1 cold-L2 time over batch sizes, sort off vs on (best of 3 alternating medians of 12 steps):")
+    for n in (1024, 2048, 4096, 8192, 16384, 32768, 65536, 200000):
+        qn = q[:n].contiguous()
+        o3 = {}
+        res = {0: [], 1: []}
+        for rep in range(3):
+            for on in (0, 1):
+                ops.set_option("sort_min_queries", 1 if on else 0)
+                res[on].append(timed(lambda: npm.query_sdf(qn, dec, out=o3), 15)[0])
+        off, on = min(res[0]), min(res[1])
+        print(f"  n {n:7d}: off {1e3 * off:8.1f} us  on {1e3 * on:8.1f} us  ({100 * (on / off - 1):+.1f} %)", flush=True)
+    ops.set_option("sort_min_queries", ops.SORT_MIN_QUERIES)
 
 # ---- 3. per-role cycle table of one profiled launch of wsq_decode_kernel<32, true, true>
 # role codes as written by wsq.cu (WS_ROLE_*) -> (name, slot names, indices of the slots that are waits)

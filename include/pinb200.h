@@ -125,7 +125,7 @@ typedef struct pinb200_query_opts {
 } pinb200_query_opts;
 
 #define PINB200_SPLIT_MIN_QUERIES 32768   /* decode-every-neighbour maps */
-#define PINB200_SPLIT_MIN_QUERIES_WF 1024 /* weighted_first maps whose decoder runs on the wgmma kernels (hidden 64, 1-2 layers,
+#define PINB200_SPLIT_MIN_QUERIES_WF 1024 /* weighted_first maps whose decoder runs on the wgmma kernel (hidden 64, 1-2 layers,
                                              F in {8,16,32}): the two-launch pipeline is faster from ~1 k queries on */
 #define PINB200_SORT_MIN_QUERIES 131072
 int64_t pinb200_query_workspace_bytes(int64_t n_queries);
@@ -133,8 +133,6 @@ int64_t pinb200_query_workspace_bytes(int64_t n_queries);
      "split_min_queries"  batch size from which the two-launch pipeline is used, both kinds of map (<= 0 restores the
                           defaults PINB200_SPLIT_MIN_QUERIES / PINB200_SPLIT_MIN_QUERIES_WF)
      "split_min_queries_wf"  the same for weighted_first maps only
-     "decode_variant"     0: phase-synchronous wgmma decode with backward MMAs (decode_umma_kernel)
-                          1: warp-specialised forward-mode decode (wsq_decode_kernel; default)
      "sort_min_queries"   batch size from which inference batches of the two-launch pipeline whose decodes all run on
                           wsq_decode_kernel are sorted spatially (Morton order of their cells) before the neighbour
                           search; 0: never (default PINB200_SORT_MIN_QUERIES).  The outputs are the same either way.

@@ -26,9 +26,10 @@ namespace pinb {
 
 // K1a of the split pipeline: phase A1 alone, at high occupancy (no decoder weights in shared memory, <= 128
 // registers): the probe rounds of ~16 resident warps per SM keep the load/store unit busy, which the fused kernel's
-// 12 warps (most of them in compute phases at any time) cannot.  One warp = one 32-query tile.  SORTED: the tiles
-// are runs of p.perm (spatially sorted queries), and the stash blocks are StashS blocks.
-template <bool SEEDS, bool SORTED>
+// 12 warps (most of them in compute phases at any time) cannot.  One warp = one 32-query tile.  COMPACT: the stash
+// blocks are StashS blocks (the decode runs on wsq_decode_kernel); with p.perm the tiles are runs of p.perm
+// (spatially sorted queries).
+template <bool SEEDS, bool COMPACT>
 __global__ void __launch_bounds__(128, 4) search_kernel(const __grid_constant__ QueryParams p) {
   extern __shared__ __align__(16) float smem[];
   uint32_t* s_delta = reinterpret_cast<uint32_t*>(smem);
@@ -39,8 +40,8 @@ __global__ void __launch_bounds__(128, 4) search_kernel(const __grid_constant__ 
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
   for (int st = blockIdx.x * nwarp + warp; st < p.n_tiles; st += gridDim.x * nwarp)
-    a1_tile<SEEDS, SORTED>(p, s_delta, (long long)st * WT, WT, lane,
-                           p.stash + (size_t)st * (SORTED ? StashS::floats : Stash::floats));
+    a1_tile<SEEDS, COMPACT>(p, s_delta, (long long)st * WT, WT, lane,
+                            p.stash + (size_t)st * (COMPACT ? StashS::floats : Stash::floats));
 }
 
 // ---------------------------------------------------------------------------
@@ -481,16 +482,9 @@ __global__ void __launch_bounds__(256) gather_kernel(const __grid_constant__ pin
   }
 }
 
-}  // namespace pinb
-
-#include "decode_umma.cuh"
-
-namespace pinb {
-
 // run-time tunables (pinb200_set_option)
 static long long g_split_min_queries = PINB200_SPLIT_MIN_QUERIES;        // decode-every-neighbour maps (mma.sync decode)
 static long long g_split_min_queries_wf = PINB200_SPLIT_MIN_QUERIES_WF;  // weighted_first maps (tensor-core decode)
-static int g_decode_variant = 1;  // 0: decode_umma_kernel (phase-synchronous, backward MMAs), 1: wsq_decode_kernel
 static long long g_sort_min_queries = PINB200_SORT_MIN_QUERIES;  // spatial sort before the search launch; 0: never
 static long long g_sort_min_queries_color = 0;                    // the same for calls with a colour head
 
@@ -632,14 +626,14 @@ static int dispatch_query(QueryParams& p, cudaStream_t stream, bool split) {
   return p.opts.weighted_first ? dispatch_query_wf<true, false>(p, stream) : dispatch_query_wf<false, false>(p, stream);
 }
 
-// K1a launch of the split pipeline
-static int launch_search(QueryParams& p, cudaStream_t stream) {
+// K1a launch of the split pipeline; `compact`: write StashS blocks
+static int launch_search(QueryParams& p, bool compact, cudaStream_t stream) {
   p.qpt = WT;
   p.n_tiles = (int)((p.n + WT - 1) / WT);
   const long long ctas = (p.n_tiles + 3) / 4;
   const int grid = (int)std::min<long long>(ctas, (long long)sm_count() * 4);
   const size_t smem = align4(p.map.n_probe) * sizeof(float);
-  if (p.perm) {
+  if (compact) {
     if (p.seeds)
       search_kernel<true, true><<<grid, 128, smem, stream>>>(p);
     else
@@ -724,47 +718,36 @@ extern "C" int pinb200_query_sdf(const pinb200_map_view* map, const pinb200_deco
   const int64_t need = pinb200_query_workspace_bytes(n);
   // weighted_first maps with a wgmma-decodable configuration: the two-launch pipeline wins from ~1 k queries on
   // (8 k queries, F = 32: 48 us vs 72 us for the fused launch; scripts/exp_small_n.py)
-  QueryParams probe{};
-  probe.dec = *sdf_dec;
-  probe.opts = *opts;
   // (training-mode batches of the mapper are value-only and tile poorly at 16-26 k rows: they keep the general threshold)
-  const long long split_min = (umma_decode_supported(probe) && !opts->training_mode) ? g_split_min_queries_wf : g_split_min_queries;
+  const long long split_min = (wsq_supported(*sdf_dec, *opts) && !opts->training_mode) ? g_split_min_queries_wf : g_split_min_queries;
   const bool split = opts->workspace && opts->workspace_bytes >= need && n >= split_min;
+  // Split calls whose decodes all run on wsq_decode_kernel write compact stash blocks (StashS) and, with d/dq, the
+  // forward-mode seeds after them; every decode of any other split call runs on query_kernel from full Stash blocks.
+  const bool compact = split && wsq_supported(*sdf_dec, *opts) && (!color_dec || wsq_supported(*color_dec, *opts));
   if (split) {
     p.stash = reinterpret_cast<float*>(opts->workspace);
-    // the warp-specialised decode takes the forward-mode seeds of d/dq from the search launch (second workspace region)
-    const bool want_seeds = g_decode_variant == 1 && umma_decode_supported(p) &&
-                            (opts->need_grad || (color_dec && opts->need_grad && out->color_grad));
-    // Large inference batches whose decodes all run on wsq_decode_kernel are searched in Morton order of their cells
-    // (2x the map resolution): the lanes of a tile then probe the same or neighbouring cells.  Their stash blocks are
-    // compact (StashS), which leaves room in the workspace for the sort (query_sort.cu); if it does not fit, the batch
-    // runs unsorted.  Calls with a colour head have their own threshold, off by default: the large one (the dense
-    // RGB-D query) comes in pixel order, already coherent, and sorting it only adds the sort (0.420 -> 0.487 ms at
-    // 307 k pixels, H100 at 400 W).
+    const bool want_seeds = compact && opts->need_grad;
+    // Large inference batches with compact stash blocks are searched in Morton order of their cells (2x the map
+    // resolution): the lanes of a tile then probe the same or neighbouring cells.  The compact blocks leave room in
+    // the workspace for the sort (query_sort.cu); if it does not fit, the batch runs unsorted.  Calls with a colour
+    // head have their own threshold, off by default: the large one (the dense RGB-D query) comes in pixel order,
+    // already coherent, and sorting it only adds the sort (0.420 -> 0.487 ms at 307 k pixels, H100 at 400 W).
     const long long sort_min = color_dec ? g_sort_min_queries_color : g_sort_min_queries;
-    bool sorted = false;
-    if (sort_min > 0 && n >= sort_min && g_decode_variant == 1 && !opts->training_mode && umma_decode_supported(p)) {
-      QueryParams c = p;
-      if (color_dec) c.dec = *color_dec;
-      if (umma_decode_supported(c)) {
-        char* base = static_cast<char*>(opts->workspace);
-        const size_t used = (size_t)p.n_tiles * (StashS::floats + (want_seeds ? Seeds::floats : 0)) * sizeof(float);
-        rc = sort_queries(query_xyz, opts->transform, n, map->resolution, base + used,
-                          (size_t)opts->workspace_bytes - used, &p.perm, (cudaStream_t)stream);
-        if (rc) return rc;
-        sorted = p.perm != nullptr;
-      }
+    if (compact && !opts->training_mode && sort_min > 0 && n >= sort_min) {
+      char* base = static_cast<char*>(opts->workspace);
+      const size_t used = (size_t)p.n_tiles * (StashS::floats + (want_seeds ? Seeds::floats : 0)) * sizeof(float);
+      rc = sort_queries(query_xyz, opts->transform, n, map->resolution, base + used,
+                        (size_t)opts->workspace_bytes - used, &p.perm, (cudaStream_t)stream);
+      if (rc) return rc;
     }
-    p.seeds = want_seeds ? p.stash + (size_t)p.n_tiles * (sorted ? StashS::floats : Stash::floats) : nullptr;
-    rc = launch_search(p, (cudaStream_t)stream);
+    p.seeds = want_seeds ? p.stash + (size_t)p.n_tiles * StashS::floats : nullptr;
+    rc = launch_search(p, compact, (cudaStream_t)stream);
     if (rc) return rc;
   }
-  // decode: wgmma tiles of 128 queries where the configuration allows it, else the warp-level mma.sync kernel
+  // decode: wgmma tiles of 128 queries where every decoder of the call allows it, else the warp-level mma.sync kernel
   p.pdl = split ? 1 : 0;  // only the launch that directly follows the search launch
   auto decode = [&](QueryParams& qp) {
-    if (split && umma_decode_supported(qp))
-      return g_decode_variant == 1 ? dispatch_wsq(qp, (cudaStream_t)stream) : dispatch_decode_umma(qp, (cudaStream_t)stream);
-    return dispatch_query(qp, (cudaStream_t)stream, split);
+    return compact ? dispatch_wsq(qp, (cudaStream_t)stream) : dispatch_query(qp, (cudaStream_t)stream, split);
   };
   rc = decode(p);
   if (rc) return rc;
@@ -799,12 +782,6 @@ extern "C" int pinb200_set_option(const char* name, int64_t value) {
     g_split_min_queries_wf = value > 0 ? value : PINB200_SPLIT_MIN_QUERIES_WF;
   } else if (key == "split_min_queries_wf") {
     g_split_min_queries_wf = value > 0 ? value : PINB200_SPLIT_MIN_QUERIES_WF;
-  } else if (key == "decode_variant") {
-    if (value < 0 || value > 1) {
-      set_error("set_option: decode_variant %lld (0: phase-synchronous wgmma decode, 1: warp-specialised)", (long long)value);
-      return PINB200_ERR_BAD_ARG;
-    }
-    g_decode_variant = (int)value;
   } else if (key == "sort_min_queries") {  // batches of at least this many queries are sorted; 0: never
     if (value < 0) {
       set_error("set_option: sort_min_queries %lld < 0", (long long)value);

@@ -47,13 +47,14 @@ struct QueryParams {
   int is_color;       // outputs go to out.color / out.color_grad instead of sdf / grad
   int n_tiles;
   int qpt;  // queries per warp tile
-  float* stash;  // split pipeline: [n_tiles][Stash::floats] workspace written by search_kernel, read by the decode launch
+  // split pipeline: [n_tiles][Stash::floats] (decode on query_kernel) or [n_tiles][StashS::floats] (decode on
+  // wsq_decode_kernel) workspace written by search_kernel, read by the decode launch
+  float* stash;
   float* seeds;  // split pipeline with d/dq on the warp-specialised decode: [n_tiles][Seeds::floats] forward-mode seeds
   int pdl;       // host only: this decode launch directly follows its search launch (programmatic dependent launch)
   QueryLayout lay;
-  // split pipeline with spatially sorted queries: perm[i] = original index of the i-th query in sorted order (the
-  // search launch then works on perm[32 st + lane] and writes the compact StashS blocks; the decode stores row
-  // results at the original index).  nullptr: queries in the caller's order, Stash blocks.
+  // search launch with spatially sorted queries (StashS blocks only): perm[i] = original index of the i-th query in
+  // sorted order; the search launch works on perm[32 st + lane].  nullptr: queries in the caller's order.
   const int32_t* perm;
 };
 
@@ -350,9 +351,9 @@ struct Stash {
   static constexpr int floats = pos + WT * 3;
 };
 static_assert(Stash::floats % 4 == 0, "stash block is copied with 16-byte accesses");
-// The block of a sorted launch (QueryParams::perm) holds only what the warp-specialised decode reads, in the order of
-// the decode's meta block (one bulk copy): neighbour ids, IDW weights, position part, and the original index of every
-// query of the tile (-1 past the end of the batch).
+// The block read by the warp-specialised decode (wsq.cu) holds only what that decode reads, in the order of its meta
+// block (one bulk copy): neighbour ids, IDW weights, position part, and the original index of every query of the
+// tile (-1 past the end of the batch).
 struct StashS {
   static constexpr int li = 0;
   static constexpr int w = li + WT * 8;
@@ -447,9 +448,9 @@ __device__ __forceinline__ void tangent_seeds(const pinb200_map_view& m, int K, 
     for (int i = 0; i < 3; ++i) sd[Seeds::P + (j * 3 + i) * WT + lane] = P[j][i];
 }
 
-// SORTED: lane `lane` works on query p.perm[q0s + lane] (per-query outputs go to that index) and `stash` is a StashS
-// block; the seeds stay in tile order.
-template <bool SEEDS = false, bool SORTED = false>
+// COMPACT: `stash` is a StashS block; with p.perm, lane `lane` works on query p.perm[q0s + lane] (per-query outputs
+// go to that index).  The seeds stay in tile order.
+template <bool SEEDS = false, bool COMPACT = false>
 __device__ __forceinline__ void a1_tile(const QueryParams& p, const uint32_t* s_delta, long long q0s, int WQ, int lane,
                                         float* stash) {
   const pinb200_map_view& m = p.map;
@@ -462,11 +463,14 @@ __device__ __forceinline__ void a1_tile(const QueryParams& p, const uint32_t* s_
   float* s_q = stash + Stash::q;
   float* s_usum = stash + Stash::usum;
   int* s_nn = reinterpret_cast<int*>(stash + Stash::nn);
-  float* s_pos = stash + (SORTED ? StashS::pos : Stash::pos);
+  float* s_pos = stash + (COMPACT ? StashS::pos : Stash::pos);
   const bool live = lane < WQ && q0s + lane < p.n;
   long long qi = q0s + lane;
-  if (SORTED) {
-    qi = live ? (long long)__ldg(p.perm + q0s + lane) : -1;
+  if (COMPACT) {
+    if (!live)
+      qi = -1;
+    else if (p.perm)
+      qi = __ldg(p.perm + q0s + lane);
     reinterpret_cast<int*>(stash + StashS::perm)[lane] = (int)qi;
   }
   float qx = 0.f, qy = 0.f, qz = 0.f;
@@ -572,14 +576,14 @@ __device__ __forceinline__ void a1_tile(const QueryParams& p, const uint32_t* s_
     if (k < K) {
       s_li[k * WT + lane] = lif[k];
       s_w[k * WT + lane] = w[k];
-      if (!SORTED) {
+      if (!COMPACT) {
         s_dx[k * WT + lane] = dx;
         s_dy[k * WT + lane] = dy;
         s_dz[k * WT + lane] = dz;
       }
     }
   }
-  if (!SORTED) {
+  if (!COMPACT) {
     s_nn[lane] = cnt;
     s_usum[lane] = usum;
     s_q[0 * WT + lane] = qx;
@@ -623,7 +627,9 @@ __device__ __forceinline__ void a1_tile(const QueryParams& p, const uint32_t* s_
 
 
 struct QueryParams;
-int dispatch_wsq(QueryParams& p, cudaStream_t stream);  // wsq.cu
+// wsq.cu: the warp-specialised decode covers weighted_first maps with a 1- or 2-layer 64-wide decoder and F in {8, 16, 32}
+bool wsq_supported(const pinb200_decoder_view& d, const pinb200_query_opts& o);
+int dispatch_wsq(QueryParams& p, cudaStream_t stream);
 void wsq_set_profile(int on);
 int wsq_read_profile(unsigned long long* host_out, int64_t count);
 int sort_queries(const float* xyz, const double* transform, long long n, float resolution, void* scratch,

@@ -1,6 +1,6 @@
-// Hopper warpgroup-MMA (wgmma) building blocks shared by the tensor-core decode kernels (decode_umma.cuh, wsq.cu):
-// shared-memory matrix descriptors of the no-swizzle canonical K-major layout, wgmma issue (operands from shared memory
-// or, for A, from registers), TF32 hi/lo split, weight staging.
+// Hopper warpgroup-MMA (wgmma) building blocks of the warp-specialised decode (wsq.cu): shared-memory matrix
+// descriptors of the no-swizzle canonical K-major layout, wgmma issue (operands from shared memory or, for A, from
+// registers), TF32 hi/lo split, weight staging.
 //
 // Accumulator fragment of a 64 x N wgmma (per warpgroup of 128 threads): warp w of the group, lane l, g = l / 4,
 // c = l % 4 holds for every 8-column block j: d[4j + 0, 1] = rows 16w + g, columns 8j + 2c, 8j + 2c + 1 and
@@ -31,17 +31,6 @@ __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.alig
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// D[64 x 16] (+)= A B^T, tf32, both operands from shared memory
-__device__ __forceinline__ void wg_mma_n16(float (&d)[8], uint64_t adesc, uint64_t bdesc, int acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %10, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n\t}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(adesc), "l"(bdesc), "r"(acc)
-      : "memory");
-}
-
 #define PINB_WG_D32                                                                                                  \
   "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, " \
   "%24, %25, %26, %27, %28, %29, %30, %31}"
@@ -51,32 +40,9 @@ __device__ __forceinline__ void wg_mma_n16(float (&d)[8], uint64_t adesc, uint64
       "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),         \
       "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
 
-// D[64 x 64] (+)= A B^T, tf32, both operands from shared memory
-__device__ __forceinline__ void wg_mma_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, int acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " PINB_WG_D32 ", %32, %33, p, 1, 1;\n\t}\n"
-      : PINB_WG_D32_OPS
-      : "l"(adesc), "l"(bdesc), "r"(acc)
-      : "memory");
-}
-
-// D[64 x 64] (+)= A B^T, tf32, A (64 x 8) from registers in the m16n8k8 A-fragment order
-// (a0: row g, k c; a1: row g + 8, k c; a2: row g, k c + 4; a3: row g + 8, k c + 4), B from shared memory
-__device__ __forceinline__ void wg_mma_n64_rs(float (&d)[32], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
-                                              uint64_t bdesc, int acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %37, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " PINB_WG_D32 ", {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}\n"
-      : PINB_WG_D32_OPS
-      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(acc)
-      : "memory");
-}
-// The same two MMAs with the descriptors advanced by compile-time k-step offsets inside the asm statement: the caller
-// keeps one base descriptor per operand live instead of one (uniform) register pair per k-step, which is what a
-// 136-register warpgroup can afford.
+// D[64 x 64] (+)= A B^T, tf32, operands from shared memory (descriptors), with the descriptors advanced by compile-time
+// k-step offsets inside the asm statement: the caller keeps one base descriptor per operand live instead of one
+// (uniform) register pair per k-step, which is what a 136-register warpgroup can afford.
 template <int AOFF, int BOFF>
 __device__ __forceinline__ void wg_mma_n64_at(float (&d)[32], uint64_t adesc, uint64_t bdesc, int acc) {
   asm volatile(
@@ -89,6 +55,8 @@ __device__ __forceinline__ void wg_mma_n64_at(float (&d)[32], uint64_t adesc, ui
       : "l"(adesc), "l"(bdesc), "r"(acc), "n"(AOFF), "n"(BOFF)
       : "memory");
 }
+// The same with A (64 x 8) from registers in the m16n8k8 A-fragment order
+// (a0: row g, k c; a1: row g + 8, k c; a2: row g, k c + 4; a3: row g + 8, k c + 4)
 template <int BOFF>
 __device__ __forceinline__ void wg_mma_n64_rs_at(float (&d)[32], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
                                                  uint64_t bdesc, int acc) {
@@ -125,19 +93,18 @@ __device__ __forceinline__ void um_split4(const float4 v, float4& hi, float4& lo
 __device__ __forceinline__ int um_a_off(int m, int c, int K) { return (m >> 3) * ((K >> 2) * UM_A_LBO) + c * UM_A_LBO + (m & 7) * 16; }
 
 // position of column c inside its 8-column k-step when the A operand comes from accumulator registers: register
-// fragment slot k (0..3) carries accumulator column 2k, slot k + 4 column 2k + 1 (see wg_mma_n64_rs)
+// fragment slot k (0..3) carries accumulator column 2k, slot k + 4 column 2k + 1 (see wg_mma_n64_rs_at)
 __device__ __forceinline__ int um_kperm(int c) { return (c & ~7) | ((c & 1) ? 4 + ((c & 7) >> 1) : ((c & 7) >> 1)); }
 
-// stage the canonical K-major B tile of `rows` x `cols`: element (r, c) = src[r][c] (or src[c][r] when `transpose`) for
-// r < rows_src, c < cols_src, zero elsewhere; `src_ld` = leading dimension of the row-major source.  `kperm` stores
-// column c at um_kperm(c), for an A operand taken from accumulator registers.
+// stage the canonical K-major B tile of `rows` x `cols`: element (r, c) = src[r][c] for r < rows_src, c < cols_src,
+// zero elsewhere; `src_ld` = leading dimension of the row-major source.  `kperm` stores column c at um_kperm(c), for an
+// A operand taken from accumulator registers.
 __device__ __forceinline__ void um_stage_weight(const float* __restrict__ src, int src_ld, int rows_src, int cols_src, int rows,
-                                                int cols, bool transpose, unsigned char* hi, unsigned char* lo,
-                                                bool kperm = false) {
+                                                int cols, unsigned char* hi, unsigned char* lo, bool kperm = false) {
   for (int e = threadIdx.x; e < rows * cols; e += blockDim.x) {
     const int r = e / cols, c = e - r * cols;
     float w = 0.f;
-    if (r < rows_src && c < cols_src) w = transpose ? __ldg(src + (size_t)c * src_ld + r) : __ldg(src + (size_t)r * src_ld + c);
+    if (r < rows_src && c < cols_src) w = __ldg(src + (size_t)r * src_ld + c);
     const float h = __uint_as_float(__float_as_uint(w) & TF32_MASK);
     const int cs = kperm ? um_kperm(c) : c;
     const int off = (r >> 3) * ((cols >> 2) * UM_W_LBO) + (cs >> 2) * UM_W_LBO + (r & 7) * 16 + (cs & 3) * 4;
@@ -149,8 +116,6 @@ __device__ __forceinline__ void um_stage_weight(const float* __restrict__ src, i
 template <int FT>
 struct UmmaDims {
   static constexpr int K0 = (FT + 3 + 7) / 8 * 8;  // decoder input width padded to the MMA k-step
-  static constexpr int N0 = (K0 + 15) / 16 * 16;   // N of the input-gradient MMA (whole 16-column blocks)
-  static constexpr int GLD = K0 + 4;               // leading dimension (floats) of the row-major input-gradient tile
 };
 
 }  // namespace pinb

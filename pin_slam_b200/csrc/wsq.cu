@@ -20,8 +20,8 @@
 // tangent rows (dx / dq_j) of the same query; tangent rows go through the same weights, without bias, and are gated
 // by the value row's ReLU pattern.  Rows 4i .. 4i+3 of a tile belong to query i, so in the accumulator fragment the
 // gate comes from the lane four rows up (one shuffle of a 32-bit mask per 64-row half).  This needs no transposed weight
-// copies, no backward MMAs, no second pass over the feature rows (the C1 phase of decode_umma_kernel) and no
-// input-gradient tile, which is what makes room for a ring of A tiles: the gathers of later tiles run under the MMA
+// copies, no backward MMAs, no second pass over the feature rows (a backward decode needs one for <d/d xbar, f_k>) and
+// no input-gradient tile, which is what makes room for a ring of A tiles: the gathers of later tiles run under the MMA
 // chain of tile t.  Without d/dq (mesher, dense RGB-D queries) a tile is 128 value rows.
 //
 // Replaces model/neural_points.py:598-731 (gathers, IDW, weighted_first), model/decoder.py:61-85,112 and the autograd
@@ -41,7 +41,7 @@ constexpr int WS_THREADS = (WS_CW + WS_GT * WS_GW) * 32;
 constexpr int WS_REG_C = 136, WS_REG_G = 120;
 static_assert((WS_CW * WS_REG_C + WS_GT * WS_GW * WS_REG_G) * 32 <= WS_THREADS * 128, "setmaxnreg pool");
 constexpr int WS_A0 = 2;       // A-tile ring slots, one per gather team
-// ring of the original query indices of a tile (sorted launches): tile i in slot i % WS_QX.  Slot i % WS_QX is
+// ring of the original query indices of a tile: tile i in slot i % WS_QX.  Slot i % WS_QX is
 // rewritten for tile i + WS_QX only after the A tile of tile i + WS_A0 was released, i.e. after every consumer warp
 // stored tile i
 constexpr int WS_QX = 2 * WS_A0;
@@ -50,7 +50,7 @@ struct WsMeta {  // float offsets inside a meta block of 32 queries, [field][k][
   static constexpr int li = 0;                   // [8][32] neighbour id | REMAP, -1 invalid
   static constexpr int w = li + WT * 8;          // [8][32] IDW weight
   static constexpr int xn = w + WT * 8;          // [3][32] sum_k w_k n_k
-  static constexpr int perm = xn + WT * 3;       // [32] original query index (sorted launches only)
+  static constexpr int perm = xn + WT * 3;       // [32] original query index, -1 past the end of the batch
   static constexpr int floats_ng = perm + WT;
   static constexpr int om = floats_ng;           // [3][8][32] d w_k / d q_j
   static constexpr int P = om + WT * 24;         // [3 j][3 i][32] d (sum_k w_k n_k)_i / d q_j
@@ -60,7 +60,7 @@ struct WsMeta {  // float offsets inside a meta block of 32 queries, [field][k][
 struct WsLayout {  // byte offsets from the dynamic shared memory base
   int w0_hi, w0_lo, w1_hi, w1_lo, b0, b1, wout, bout;
   int a0, a0_half, a0_stride;  // ring of A tiles: slot s = [a0 + s*stride: hi | + half: lo]
-  int qidx;                    // [WS_QX][128] original query index of every tile row's query (sorted launches)
+  int qidx;                    // [WS_QX][128] original query index of every tile row's query
   int meta, meta_stride, n_meta;
   int bars, total;
 };
@@ -74,8 +74,7 @@ constexpr int WSB_A0_FULL = 0, WSB_A0_EMPTY = WSB_A0_FULL + WS_A0, WSB_META_FULL
 // pinb200_debug_read("ws_profile", ...).  The last slot of every warp holds its role code (WS_ROLE_*), so that a
 // reader of the counters (scripts/exp_decode.py) follows the kernel's role layout.
 constexpr int WS_PROF_SLOTS = 8;
-// C consumer warps, G gather warps that also fill the meta ring (codes 2 and 3 stood for gather-only warps and
-// separate loader warps, an earlier layout that exp_decode.py still reads)
+// C consumer warps, G gather warps that also fill the meta ring
 constexpr int WS_ROLE_C = 1, WS_ROLE_G = 4;
 constexpr int WS_PROF_CTAS = 132;  // one CTA per SM of an H100 SXM
 __device__ unsigned long long g_ws_prof[WS_PROF_CTAS * (WS_THREADS / 32) * WS_PROF_SLOTS];
@@ -151,7 +150,7 @@ __device__ __forceinline__ void ws_arrive(uint32_t bar) {
 static_assert(WsMeta::P - WsMeta::om == Seeds::P - Seeds::om && WsMeta::floats_g - WsMeta::om == Seeds::floats,
               "the seed block of the search launch is copied verbatim into the meta block");
 static_assert(WsMeta::xn == StashS::pos && WsMeta::perm == StashS::perm && WsMeta::floats_ng == StashS::floats,
-              "a sorted launch's stash block is the head of the meta block (one bulk copy)");
+              "the stash block is the head of the meta block (one bulk copy)");
 
 // fn(std::integral_constant<int, s>) for s = 0 .. N-1: a k-step loop whose step is a compile-time constant
 template <typename Fn, int... S>
@@ -218,8 +217,8 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
     }
     asm volatile("fence.mbarrier_init.release.cluster;");
   }
-  um_stage_weight(p.dec.w[0], D, H, D, H, K0, false, sm + lay.w0_hi, sm + lay.w0_lo);
-  if (L > 1) um_stage_weight(p.dec.w[1], H, H, H, H, H, false, sm + lay.w1_hi, sm + lay.w1_lo, true);
+  um_stage_weight(p.dec.w[0], D, H, D, H, K0, sm + lay.w0_hi, sm + lay.w0_lo);
+  if (L > 1) um_stage_weight(p.dec.w[1], H, H, H, H, H, sm + lay.w1_hi, sm + lay.w1_lo, true);
   __syncthreads();
   // the layer-0 bias rides on the MMA: input column D is 1 for value rows (0 for tangent rows), weight column D = b0
   static_assert(D < K0, "a spare (padding) input column carries the bias");
@@ -321,8 +320,8 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       out_chstride = 3;
     }
     // value rows write the prediction, tangent rows one component of its gradient; lane c == r of the quad writes row r.
-    // Tile i holds queries T * QT .. in search order; a sorted launch maps them to their original index through the
-    // index ring the gather team filled (shared memory: no global load on this path)
+    // Tile i holds queries T * QT .. in search order, mapped to their original index through the index ring the
+    // gather team filled (shared memory: no global load on this path)
     const int* s_qidx = reinterpret_cast<const int*>(sm + lay.qidx);
     auto store = [&](long long T, int i, float (&o)[2][4]) {
 #pragma unroll
@@ -342,9 +341,8 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
           for (int ch = 0; ch < 4; ++ch) o[r][ch] = fmaf(bsel, s_bout[ch], o[r][ch]) * p.dec.out_scale;
         }
         const int row = 64 * h + 16 * wq + g8 + 8 * r, qrow = GRAD ? (row >> 2) : row;
-        long long qi = T * QT + qrow;
-        if (c == r && qi < p.n) {
-          if (p.perm) qi = s_qidx[(i % WS_QX) * QT + qrow];
+        if (c == r && T * QT + qrow < p.n) {  // the tail of the last tile carries no valid index
+          const long long qi = s_qidx[(i % WS_QX) * QT + qrow];
           if (out_base) {
             float* dst = out_base + qi * out_qstride;
 #pragma unroll
@@ -429,8 +427,9 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
     // passes of ONE warp was tried: it spills inside the loop at 120 registers and lost 5 %.)
     //
     // The teams also fill the meta ring: TMA bulk copies (cp.async.bulk, completion counted in bytes on the block's
-    // "full" mbarrier; no thread touches the data) of what search_kernel wrote for a 32-query block -- neighbour ids +
-    // IDW weights (2 KB), position part (384 B) and, with d/dq, the forward-mode seeds (4.1 KB).  Block blk + MB of the
+    // "full" mbarrier; no thread touches the data) of what search_kernel wrote for a 32-query block -- the StashS block
+    // (2.5 KB: neighbour ids, IDW weights, position part, original query indices) and, with d/dq, the forward-mode
+    // seeds (4.1 KB).  Block blk + MB of the
     // ring belongs to the same team as block blk, so a team refills its own slots: position j of the team's stream of
     // meta blocks takes the slot of position j - MD, and before it works on position j one warp of the team (in
     // turn) issues position j + PF, whose slot the team left two positions ago.
@@ -458,16 +457,9 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       const long long st = T * BPT + b;  // stash block
       if (st < n_blocks) {
         if (ws_elect()) {
-          constexpr uint32_t B_LW = 2 * WT * 8 * 4, B_XN = 3 * WT * 4, B_S = StashS::floats * 4, B_SD = Seeds::floats * 4;
-          if (p.perm) {  // li | w | pos | perm: one copy
-            ws_arrive_expect_tx(full, B_S + (GRAD ? B_SD : 0u));
-            ws_bulk_g2s(mt, p.stash + (size_t)st * StashS::floats, B_S, full);
-          } else {
-            const float* sb = p.stash + (size_t)st * Stash::floats;
-            ws_arrive_expect_tx(full, B_LW + B_XN + (GRAD ? B_SD : 0u));
-            ws_bulk_g2s(mt + WsMeta::li, sb + Stash::li, B_LW, full);  // li | w are adjacent in both layouts
-            ws_bulk_g2s(mt + WsMeta::xn, sb + Stash::pos, B_XN, full);
-          }
+          constexpr uint32_t B_S = StashS::floats * 4, B_SD = Seeds::floats * 4;
+          ws_arrive_expect_tx(full, B_S + (GRAD ? B_SD : 0u));
+          ws_bulk_g2s(mt, p.stash + (size_t)st * StashS::floats, B_S, full);  // li | w | pos | perm: one copy
           if (GRAD) ws_bulk_g2s(mt + WsMeta::om, p.seeds + (size_t)st * Seeds::floats, B_SD, full);
         }
       } else {  // tail of the last value-only tile: a block without neighbours
@@ -571,7 +563,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
           slot_free = true;
         }
         // the tile's original query indices, for the consumers' stores (the meta slot is refilled before they store)
-        if (p.perm && (b % WS_GW) == gw)
+        if ((b % WS_GW) == gw)
           reinterpret_cast<int*>(sm + lay.qidx)[(i % WS_QX) * QT + b * WT + lane] = reinterpret_cast<const int*>(mt + WsMeta::perm)[lane];
         // position part (columns F .. F+2) and zero padding of the rows: thread per row
         if (GRAD || (b % WS_GW) == gw) {
@@ -683,6 +675,12 @@ static int launch_wsq(QueryParams& p, cudaStream_t stream) {
     return PINB200_ERR_CUDA;
   }
   return check_launch("wsq_decode_kernel");
+}
+
+bool wsq_supported(const pinb200_decoder_view& d, const pinb200_query_opts& o) {
+  const int F = d.in_dim - 3;
+  return o.weighted_first && d.hidden_dim == 64 && d.n_hidden >= 1 && d.n_hidden <= 2 && (F == 8 || F == 16 || F == 32) &&
+         o.nn_k <= KREG;
 }
 
 int dispatch_wsq(QueryParams& p, cudaStream_t stream) {

@@ -23,8 +23,8 @@ def uses_split(n: int, weighted_first: bool, dec=None, training_mode: bool = Fal
 
 
 def set_option(name: str, value: int) -> None:
-    """Process-wide tunables of the query path (pinb200_set_option): "split_min_queries", "decode_variant",
-    "sort_min_queries" (0: never sort), "sort_min_queries_color" (calls with a colour head; default 0)."""
+    """Process-wide tunables of the query path (pinb200_set_option): "split_min_queries", "sort_min_queries"
+    (0: never sort), "sort_min_queries_color" (calls with a colour head; default 0)."""
     global SPLIT_MIN_QUERIES, SPLIT_MIN_QUERIES_WF
     _lib.check(_lib.load().pinb200_set_option(name.encode(), int(value)), "pinb200_set_option")
     if name == "split_min_queries":

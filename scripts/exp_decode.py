@@ -1,9 +1,9 @@
 """Where the time of K1 (search launch + decode launch) goes at BASELINE cfg2 (200k queries, K = 8, F = 32, 2 x 64
 decoder, d sdf / dq), the headline workload of bench.py:
 
-  1. A/B of the two decode variants of the split pipeline (CUDA events, L2 flushed before every step)
-  2. per-kernel device time per step of the default variant (torch.profiler with CUDA activities, a run of its own);
-     with --out DIR the trace goes to DIR/exp_decode_trace.json
+  1. K1 time with d/dq and value-only, library defaults (CUDA events, L2 flushed before every step)
+  2. per-kernel device time per step (torch.profiler with CUDA activities, a run of its own); with --out DIR the trace
+     goes to DIR/exp_decode_trace.json
   3. per-role cycle table of wsq_decode_kernel: per warp, clock deltas of the phases of its role, summed over one
      profiled launch (ws_profile); the role of every warp is read from the counters, so the table follows the kernel
 
@@ -14,7 +14,7 @@ queries pre-permuted in Python into Morton order of their 0.4 m cells: the best 
 could reach, without its cost.  --sort-sweep times K1 with the sort off and on over batch sizes (CUDA events, L2
 flushed before every step), to place the default of sort_min_queries.
 
-python scripts/exp_decode.py [variant ...] [--steps N] [--out DIR] [--presorted] [--sort-sweep]"""
+python scripts/exp_decode.py [--steps N] [--out DIR] [--presorted] [--sort-sweep]"""
 import argparse
 import os
 import sys
@@ -29,7 +29,6 @@ from pin_slam_b200.model import Decoder
 from pin_slam_b200.synthetic import build_map, surface_queries
 
 ap = argparse.ArgumentParser()
-ap.add_argument("variants", type=int, nargs="*", default=[0, 1])
 ap.add_argument("--steps", type=int, default=20, help="steps of the profiled run")
 ap.add_argument("--out", default=None, help="directory for the profiler trace")
 ap.add_argument("--presorted", action="store_true",
@@ -44,7 +43,6 @@ npm = build_map(cfg, n_surface=3_000_000, seed=0, extent=80.0)
 torch.manual_seed(42)
 dec = Decoder(cfg, cfg.geo_mlp_hidden_dim, cfg.geo_mlp_level, 1)
 q = surface_queries(npm, 200000, seed=1, sigma=0.1)
-ref = None
 
 
 def timed(fn, n=10):
@@ -61,33 +59,14 @@ def timed(fn, n=10):
     return ts[len(ts) // 2], ts[0]
 
 
-# ---- 1. decode variants
-for variant in args.variants:
-    ops.set_option("decode_variant", variant)
-    out = {}
-    ts = []
-    for it in range(10):
-        flush.zero_()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        npm.query_sdf(q, dec, out=out)
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b))
-    ts = sorted(ts[3:])
-    line = f"variant {variant}: K1 (search + decode) cold-L2 median {ts[len(ts) // 2]:.4f} ms, min {ts[0]:.4f} ms"
-    if ref is None:
-        ref = {k: v.clone() for k, v in out.items() if torch.is_tensor(v) and not k.startswith("_")}
-    else:
-        ds = (out["sdf"] - ref["sdf"]).abs().max().item()
-        dg = (out["grad"] - ref["grad"]).abs().max().item()
-        line += f"; vs first variant: max |d sdf| {ds:.3e}, max |d grad| {dg:.3e} (|grad| mean {ref['grad'].abs().mean().item():.3e})"
-    print(line, flush=True)
-    o2 = {}
-    med, mn = timed(lambda: npm.query_sdf(q, dec, need_grad=False, out=o2))
-    print(f"variant {variant}: value-only (need_grad=False) cold-L2 median {med:.4f} ms, min {mn:.4f} ms", flush=True)
+# ---- 1. K1 with d/dq and value-only
+o1 = {}
+med, mn = timed(lambda: npm.query_sdf(q, dec, out=o1))
+print(f"K1 (search + decode) cold-L2 median {med:.4f} ms, min {mn:.4f} ms", flush=True)
+med, mn = timed(lambda: npm.query_sdf(q, dec, need_grad=False, out=o1))
+print(f"value-only (need_grad=False) cold-L2 median {med:.4f} ms, min {mn:.4f} ms", flush=True)
 
-# ---- 2. per-kernel device time of the warp-specialised decode variant (the default)
+# ---- 2. per-kernel device time
 from torch.profiler import ProfilerActivity, profile
 
 def morton_presort(x, cell=0.4):
@@ -133,7 +112,6 @@ def kernel_table(qq, label, trace_name):
 
 
 K1_KERNELS = ("search_kernel", "wsq_decode_kernel", "sort_key_kernel", "DeviceScan", "sort_scatter_kernel", "Memset")
-ops.set_option("decode_variant", 1)
 out = kernel_table(q, "random queries, library defaults", "exp_decode_trace.json")
 if args.presorted:
     ops.set_option("sort_min_queries", 0)
@@ -158,8 +136,6 @@ if args.sort_sweep:
 # role codes as written by wsq.cu (WS_ROLE_*) -> (name, slot names, indices of the slots that are waits)
 ROLES = {
     1: ("C consumer", ["wait_A", "layer0", "layer1", "last+out"], {0}),
-    2: ("G gather", ["wait_A_free", "wait_meta", "issue_loads", "reduce+store", "pos+fence"], {0, 1}),
-    3: ("L loader", ["wait_meta_free", "copies"], {0}),
     4: ("G gather + meta refill", ["wait_A_free", "wait_meta", "issue_loads", "reduce+store", "pos+fence",
                                    "meta_refill", "wait_search"], {0, 1, 6}),
 }

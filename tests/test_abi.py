@@ -99,7 +99,7 @@ def test_install_registers_reference_module_names():
                    "pin_slam_b200.utils.mapper"]
 
 
-def test_run_time_options_and_split_rule():
+def test_run_time_options_split_rule_and_workspace_sizes():
     """pinb200_set_option / ops.uses_split (no GPU needed: host-side state only): known options are accepted and
     mirrored in ops, unknown ones and out-of-range values fail loudly, workspace sizes cover stash + seeds."""
     from pin_slam_b200 import _lib, ops
@@ -117,10 +117,8 @@ def test_run_time_options_and_split_rule():
     ops.set_option("split_min_queries_wf", 4096)
     assert not ops.uses_split(2048, True)
     ops.set_option("split_min_queries_wf", 0)
-    for variant in (0, 1):
-        ops.set_option("decode_variant", variant)
     with pytest.raises(RuntimeError):
-        ops.set_option("decode_variant", 7)
+        ops.set_option("decode_variant", 1)  # one decode per configuration: no option selects it
     with pytest.raises(RuntimeError):
         ops.set_option("no_such_option", 1)
     # 32 queries per tile: stash (1536 floats) + forward-mode seeds (1056 floats)

@@ -227,19 +227,29 @@ def test_fused_query_vs_oracle_synthetic(F, K, L, wf, pgo, C):
     assert torch.equal(out2["sdf"], out["sdf"])
 
 
-@pytest.mark.parametrize("variant", [1, 0])
 @pytest.mark.parametrize("F,K,L,pgo,color,leaky", [(32, 8, 2, False, False, False), (8, 6, 1, False, True, False),
                                                    (16, 4, 2, True, False, False), (32, 8, 1, True, True, True),
                                                    (8, 3, 2, False, False, True)])
-def test_split_pipeline_decoders_vs_oracle(F, K, L, pgo, color, leaky, variant):
-    """The two-launch pipeline (search_kernel -> tensor-core decode) forced onto oracle-sized batches: the
-    warp-specialised forward-mode decode (variant 1, default) and the phase-synchronous decode with backward MMAs
-    (variant 0) against the oracle -- value, d/dq, colour head + its Jacobian, ragged last tile, queries without
-    neighbours, and the value-only launch (128-query tiles)."""
+@pytest.mark.parametrize("sort", [False, True])
+def test_split_pipeline_decoders_vs_oracle(F, K, L, pgo, color, leaky, sort):
+    """The two-launch pipeline (search_kernel -> warp-specialised tensor-core decode on compact stash blocks) forced
+    onto oracle-sized batches, in the caller's query order and spatially sorted, against the oracle -- value, d/dq,
+    colour head + its Jacobian, ragged last tile, queries without neighbours, and the value-only launch (128-query
+    tiles)."""
+    _check_split_pipeline_vs_oracle(F, K, L, L, pgo, color, leaky, sort)
+
+
+def test_split_pipeline_mixed_decoder_depths_vs_oracle():
+    """A call whose colour decoder (3 hidden layers) has no warp-specialised decode while its SDF decoder (2 layers)
+    has one: both decodes run on query_kernel from full stash blocks."""
+    _check_split_pipeline_vs_oracle(32, 8, 2, 3, False, True, False, False)
+
+
+def _check_split_pipeline_vs_oracle(F, K, L, color_L, pgo, color, leaky, sort):
     m = synthetic_map(n_surface=60000, seed=F + K, resolution=0.4, buffer_size=200003, feature_dim=F, color=color,
                       after_pgo=pgo, local_radius=14.0, diff_td=3.0)
     dec = po.make_decoder(F + 3, 64, L, 1, 0.044, seed=3)
-    cdec = po.make_decoder(F + 3, 64, L, 3, 1.0, seed=4) if color else None
+    cdec = po.make_decoder(F + 3, 64, color_L, 3, 1.0, seed=4) if color else None
     if leaky:
         dec.leaky = True
         if cdec is not None:
@@ -254,14 +264,16 @@ def test_split_pipeline_decoders_vs_oracle(F, K, L, pgo, color, leaky, variant):
     ch = decoder_handle_from_oracle(cdec, sigmoid_out=True) if color else None
     o = ops()
     o.set_option("split_min_queries", 1)
-    o.set_option("decode_variant", variant)
+    o.set_option("sort_min_queries", 1 if sort else 0)
+    o.set_option("sort_min_queries_color", 1 if sort else 0)
     try:
         out = o.query_sdf(mh, dh, q.cuda(), nn_k=K, weighted_first=True, need_grad=True, color_dec=ch, color_grad=color)
         out2 = o.query_sdf(mh, dh, q.cuda(), nn_k=K, weighted_first=True, need_grad=False, color_dec=ch)
         torch.cuda.synchronize()
     finally:
         o.set_option("split_min_queries", 0)
-        o.set_option("decode_variant", 1)
+        o.set_option("sort_min_queries", o.SORT_MIN_QUERIES)
+        o.set_option("sort_min_queries_color", 0)
     assert np.array_equal(out["nn_count"].cpu().numpy(), ref["nn_count"].numpy())
     assert_sdf_close(out["sdf"].cpu(), ref["sdf"], dec.sdf_scale)
     assert_sdf_close(out2["sdf"].cpu(), ref["sdf"], dec.sdf_scale)
@@ -273,7 +285,6 @@ def test_split_pipeline_decoders_vs_oracle(F, K, L, pgo, color, leaky, variant):
         assert_sdf_close(out2["color"].cpu(), ref["color"], 1.0)
         cscale = float(ref["color_grad"].abs().mean()) + 1e-12
         assert_rel_close(out["color_grad"].cpu(), ref["color_grad"], 1e-4, cscale, r64["color_grad"], kink_rows=8)
-
 
 
 def test_fused_transform_matches_pretransformed():

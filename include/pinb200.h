@@ -202,7 +202,9 @@ int pinb200_gather_features(const pinb200_map_view* map, const float* feat, cons
                             int32_t weighted_first, float* out, void* stream);
 
 /* Flat layout of decoder gradients / Adam state used by K2/K3:
- * [w0 | b0 | w1 | b1 | ... | w_out | b_out], each row-major as in the view. */
+ * [w0 | b0 | w1 | b1 | ... | w_out | b_out], each row-major as in the view.  A bias that is NULL in the view
+ * (mlp_bias_on False) has no block: a decoder without biases is [w0 | w1 | ... | w_out], which is what
+ * Decoder.flat_parameters() builds.  The count is of the blocks present. */
 int64_t pinb200_decoder_param_count(const pinb200_decoder_view* dec);
 
 /* K2 -- backward of one map-training batch.  Given the saved kNN ids/weights of

@@ -417,8 +417,9 @@ class DecoderParams:
         )
 
 
-def make_decoder(in_dim, hidden_dim, hidden_level, out_dim, sdf_scale, seed=0, device="cpu"):
-    """nn.Linear default init (kaiming_uniform a=sqrt(5) -> U(-1/sqrt(in), 1/sqrt(in)))."""
+def make_decoder(in_dim, hidden_dim, hidden_level, out_dim, sdf_scale, seed=0, device="cpu", bias=True):
+    """nn.Linear default init (kaiming_uniform a=sqrt(5) -> U(-1/sqrt(in), 1/sqrt(in))).  `bias=False`
+    (mlp_bias_on False, model/decoder.py:43-51): the biases are zero, which is the same forward pass as none."""
     g = torch.Generator().manual_seed(seed)
     hs = []
     d = in_dim
@@ -426,12 +427,12 @@ def make_decoder(in_dim, hidden_dim, hidden_level, out_dim, sdf_scale, seed=0, d
         bound = 1.0 / math.sqrt(d)
         w = (torch.rand(hidden_dim, d, generator=g) * 2 - 1) * bound
         b = (torch.rand(hidden_dim, generator=g) * 2 - 1) * bound
-        hs.append((w.to(device), b.to(device)))
+        hs.append((w.to(device), (b if bias else torch.zeros_like(b)).to(device)))
         d = hidden_dim
     bound = 1.0 / math.sqrt(d)
     wo = (torch.rand(out_dim, d, generator=g) * 2 - 1) * bound
     bo = (torch.rand(out_dim, generator=g) * 2 - 1) * bound
-    return DecoderParams(hs, (wo.to(device), bo.to(device)), sdf_scale)
+    return DecoderParams(hs, (wo.to(device), (bo if bias else torch.zeros_like(bo)).to(device)), sdf_scale)
 
 
 def decoder_mlp(p: DecoderParams, x: torch.Tensor) -> torch.Tensor:
@@ -498,6 +499,9 @@ def query_sdf(
     sdf = decoder_sdf(dec, geo)
     sdf_std = torch.zeros(coord.shape[0], device=coord.device, dtype=coord.dtype)
     if not weighted_first:
+        # [N,K,1]; decoder_sdf's squeeze(1) drops the K axis when K = 1, and the reference's [N,1] * [N,1,1] would
+        # broadcast to [N,N,1] -- the K > 1 semantics apply
+        sdf = sdf.reshape(w.shape)
         mean = torch.sum(sdf * w, dim=1)  # [N,1]
         var = torch.sum(w * (sdf - mean.unsqueeze(-1)) ** 2, dim=1)
         sdf_std = torch.sqrt(var).squeeze(1).detach()

@@ -43,11 +43,12 @@ extern "C" const char* pinb200_last_error(void) { return pinb::g_err; }
 
 extern "C" int64_t pinb200_decoder_param_count(const pinb200_decoder_view* d) {
   if (!d) return -1;
+  // [w0 | b0 | w1 | b1 | ... | w_out | b_out]; a NULL bias (mlp_bias_on False) has no slot
   int64_t n = 0;
   for (int l = 0; l < d->n_hidden; ++l) {
     const int in = l == 0 ? d->in_dim : d->hidden_dim;
-    n += (int64_t)d->hidden_dim * in + d->hidden_dim;
+    n += (int64_t)d->hidden_dim * in + (d->b[l] ? d->hidden_dim : 0);
   }
-  n += (int64_t)d->out_dim * d->hidden_dim + d->out_dim;
+  n += (int64_t)d->out_dim * d->hidden_dim + (d->b_out ? d->out_dim : 0);
   return n;
 }

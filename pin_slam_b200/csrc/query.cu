@@ -626,24 +626,20 @@ static int dispatch_query(QueryParams& p, cudaStream_t stream, bool split) {
   return p.opts.weighted_first ? dispatch_query_wf<true, false>(p, stream) : dispatch_query_wf<false, false>(p, stream);
 }
 
-// K1a launch of the split pipeline; `compact`: write StashS blocks
+// K1a launch of the split pipeline; `compact`: write StashS blocks.  Only wsq_decode_kernel reads the forward-mode
+// seeds, and it reads compact blocks, so p.seeds is set only with `compact`.
 static int launch_search(QueryParams& p, bool compact, cudaStream_t stream) {
   p.qpt = WT;
   p.n_tiles = (int)((p.n + WT - 1) / WT);
   const long long ctas = (p.n_tiles + 3) / 4;
   const int grid = (int)std::min<long long>(ctas, (long long)sm_count() * 4);
   const size_t smem = align4(p.map.n_probe) * sizeof(float);
-  if (compact) {
-    if (p.seeds)
-      search_kernel<true, true><<<grid, 128, smem, stream>>>(p);
-    else
-      search_kernel<false, true><<<grid, 128, smem, stream>>>(p);
-  } else {
-    if (p.seeds)
-      search_kernel<true, false><<<grid, 128, smem, stream>>>(p);
-    else
-      search_kernel<false, false><<<grid, 128, smem, stream>>>(p);
-  }
+  if (!compact)
+    search_kernel<false, false><<<grid, 128, smem, stream>>>(p);
+  else if (p.seeds)
+    search_kernel<true, true><<<grid, 128, smem, stream>>>(p);
+  else
+    search_kernel<false, true><<<grid, 128, smem, stream>>>(p);
   return check_launch("search_kernel");
 }
 

@@ -39,11 +39,27 @@ struct TrainParams {
   const float* knn_w;
   const float* dl;  // [N, out_dim] d loss / d decoder output (after out_scale / sigmoid)
   long long n;
-  int K, wf, n_tiles, qpt, n_param;
+  // n_acc: length of the per-CTA shared-memory gradient accumulator, laid out [w0 | b0 | w1 | b1 | ... | w_out | b_out]
+  // with a slot for every bias whether the decoder has it or not (the bias sums are computed either way)
+  int K, wf, n_tiles, qpt, n_acc;
   float* grad_feat;
-  float* grad_dec;
+  // where each parameter block's gradient goes in the caller's flat gradient vector, whose layout has no slot for an
+  // absent bias (pinb200_decoder_param_count); NULL: the bias is absent and its partial sums are dropped
+  float* gd_w[PINB200_MAX_HIDDEN_LAYERS];
+  float* gd_b[PINB200_MAX_HIDDEN_LAYERS];
+  float* gd_wout;
+  float* gd_bout;
   TrainLayout lay;
 };
+
+// adds this CTA's partial sums of one parameter block (shared memory) to its block of the flat gradient vector
+__device__ __forceinline__ void flush_block(const float* src, int count, float* dst, int tid) {
+  if (!dst) return;
+  for (int e = tid; e < count; e += TILE) {
+    const float v = src[e];
+    if (v != 0.f) atomicAdd(dst + e, v);
+  }
+}
 
 // dW[j][i] += sum_r G[j][r] * A[i][r]; db[j] += sum_r G[j][r]   (thread-owned 4 x NI blocks)
 template <int NI>
@@ -102,10 +118,10 @@ __global__ void __launch_bounds__(TILE, PINB_K2_MIN_CTAS) train_bwd_kernel(const
   uint64_t* s_mask = reinterpret_cast<uint64_t*>(smem + p.lay.mask);
 
   stage_decoder(p.dec, p.lay.dec, smem, DP, true);
-  for (int e = tid; e < p.n_param; e += TILE) s_dW[e] = 0.f;
+  for (int e = tid; e < p.n_acc; e += TILE) s_dW[e] = 0.f;
   __syncthreads();
 
-  // offsets of each parameter block in the flat gradient layout
+  // offsets of each parameter block in the accumulator
   int off_w[PINB200_MAX_HIDDEN_LAYERS], off_b[PINB200_MAX_HIDDEN_LAYERS];
   int off = 0;
 #pragma unroll
@@ -352,10 +368,12 @@ __global__ void __launch_bounds__(TILE, PINB_K2_MIN_CTAS) train_bwd_kernel(const
     }
     __syncthreads();
   }
-  for (int e = tid; e < p.n_param; e += TILE) {
-    const float v = s_dW[e];
-    if (v != 0.f) atomicAdd(p.grad_dec + e, v);
+  for (int l = 0; l < L; ++l) {
+    flush_block(s_dW + off_w[l], H * (l == 0 ? D : H), p.gd_w[l], tid);
+    flush_block(s_dW + off_b[l], H, p.gd_b[l], tid);
   }
+  flush_block(s_dW + off_wout, OC * H, p.gd_wout, tid);
+  flush_block(s_dW + off_bout, OC, p.gd_bout, tid);
 }
 
 }  // namespace pinb
@@ -375,7 +393,7 @@ static int launch_train(TrainParams& p, cudaStream_t stream) {
   l.h = o;
   o += align4(p.dec.n_hidden * H * ACT_LD);
   l.dW = o;
-  o += align4(p.n_param);
+  o += align4(p.n_acc);
   l.go = o;
   o += TILE * 4;
   l.idx = o;
@@ -463,9 +481,24 @@ extern "C" int pinb200_train_backward(const pinb200_map_view* map, const pinb200
   p.wf = weighted_first;
   p.qpt = weighted_first ? TILE : TILE / nn_k;
   p.n_tiles = (int)((n + p.qpt - 1) / p.qpt);
-  p.n_param = (int)pinb200_decoder_param_count(dec);
   p.grad_feat = grad_feat;
-  p.grad_dec = grad_dec;
+  {
+    const int H = dec->hidden_dim;
+    int acc = 0;
+    float* g = grad_dec;
+    for (int l = 0; l < dec->n_hidden; ++l) {
+      const int nw = H * (l == 0 ? dec->in_dim : H);
+      p.gd_w[l] = g;
+      g += nw;
+      p.gd_b[l] = dec->b[l] ? g : nullptr;
+      if (dec->b[l]) g += H;
+      acc += nw + H;
+    }
+    p.gd_wout = g;
+    g += dec->out_dim * H;
+    p.gd_bout = dec->b_out ? g : nullptr;
+    p.n_acc = acc + dec->out_dim * H + dec->out_dim;
+  }
   const int D = dec->in_dim;
   cudaStream_t st = (cudaStream_t)stream;
   {

@@ -111,12 +111,11 @@ __global__ void __launch_bounds__(TILE, train_mma_min_ctas<FT, LT>()) train_bwd_
   float* s_w = smem + lay.w;
 
   stage_mma_decoder(p.dec, lay.dec, smem);
-  for (int e = tid; e < p.n_param; e += TILE) s_dW[e] = 0.f;
+  for (int e = tid; e < p.n_acc; e += TILE) s_dW[e] = 0.f;
   __syncthreads();
 
-  // flat gradient layout [w0 | b0 | (w1 | b1) | w_out | b_out]
-  const int off_w0 = 0, off_b0 = H * D;
-  const int off_w1 = off_b0 + H, off_b1 = off_w1 + H * H;
+  // accumulator layout [w0 | b0 | (w1 | b1) | w_out | b_out] (TrainParams::n_acc)
+  const int off_b0 = H * D, off_b1 = off_b0 + H + H * H;
   const int off_wout = LT == 1 ? off_b0 + H : off_b1 + H, off_bout = off_wout + OC * H;
 
   float dacc0[KT0][4];
@@ -385,13 +384,13 @@ __global__ void __launch_bounds__(TILE, train_mma_min_ctas<FT, LT>()) train_bwd_
   }
 
   // ---------------- flush the decoder gradients ----------------
-  flush_slab<KT0>(dacc0, p.grad_dec + off_w0, warp * 16, D, lane);
-  if constexpr (LT == 2) flush_slab<8>(dacc1, p.grad_dec + off_w1, warp * 16, H, lane);
+  flush_slab<KT0>(dacc0, p.gd_w[0], warp * 16, D, lane);
+  if constexpr (LT == 2) flush_slab<8>(dacc1, p.gd_w[1], warp * 16, H, lane);
   __syncthreads();
-  for (int e = tid; e < p.n_param; e += TILE) {
-    const float v = s_dW[e];
-    if (v != 0.f) atomicAdd(p.grad_dec + e, v);
-  }
+  flush_block(s_dW + off_b0, H, p.gd_b[0], tid);
+  if constexpr (LT == 2) flush_block(s_dW + off_b1, H, p.gd_b[1], tid);
+  flush_block(s_dW + off_wout, OC * H, p.gd_wout, tid);
+  flush_block(s_dW + off_bout, OC, p.gd_bout, tid);
 }
 
 template <int FT, int LT>
@@ -405,7 +404,7 @@ static int launch_train_mma(TrainParams& p, cudaStream_t stream) {
   l.h = o;
   o += LT * TILE * LDH;
   l.dW = o;
-  o += align4i(p.n_param);
+  o += align4i(p.n_acc);
   l.go = o;
   o += TILE * 4;
   l.idx = o;

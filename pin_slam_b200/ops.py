@@ -165,9 +165,20 @@ class DecoderHandle:
         v.leaky_relu = int(bool(leaky))
         v.sigmoid_out = int(bool(sigmoid_out))
         self.view = v
+        self._n_param = None
 
     def param_count(self):
-        return int(_lib.load().pinb200_decoder_param_count(C.byref(self.view)))
+        """Length of the flat parameter layout (pinb200_decoder_param_count): absent biases have no slot."""
+        if self._n_param is None:
+            self._n_param = int(_lib.load().pinb200_decoder_param_count(C.byref(self.view)))
+        return self._n_param
+
+    def check_flat(self, **tensors):
+        """The kernels read and write exactly param_count() floats of every flat decoder vector."""
+        n = self.param_count()
+        for name, t in tensors.items():
+            if t.numel() != n:
+                raise RuntimeError(f"pin_slam_b200: {name} holds {t.numel()} floats, the decoder has {n} parameters")
 
 
 def _query_args(xyz, nn_k, weighted_first, training_mode, need_grad, color_dec, color_grad, transform, save_knn,
@@ -311,6 +322,7 @@ def train_backward(mh: MapHandle, dec: DecoderHandle, feat, xyz, knn_idx, knn_we
                    grad_feat, grad_dec):
     lib = _lib.load()
     n, k = knn_idx.shape
+    dec.check_flat(grad_dec=grad_dec)
     rc = lib.pinb200_train_backward(C.byref(mh.view), C.byref(dec.view), _ptr(feat, torch.float32),
                                     _ptr(xyz, torch.float32), _ptr(knn_idx, torch.int32),
                                     _ptr(knn_weight, torch.float32), _ptr(dloss_dout, torch.float32), n, k,
@@ -412,6 +424,7 @@ def map_iterations(mh: MapHandle, dec: DecoderHandle, n_iter: int, *, nn_k, weig
     """The geometry-only training loop of Mapper.mapping in ONE host call (pinb200_map_iterations).
     `index` [n_iter, bs] int64 are the pre-drawn batch indices; scratch buffers live in `work`."""
     lib = _lib.load()
+    dec.check_flat(dec_flat=dec_flat, grad_dec=grad_dec, m_dec=m_dec, v_dec=v_dec)
     mh.ensure_records()
     bs = index.shape[1]
     dev = index.device

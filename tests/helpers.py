@@ -1,4 +1,13 @@
-"""Shared test helpers: golden-fixture loading and seeded synthetic maps."""
+"""Shared test helpers: golden-fixture loading, seeded synthetic maps and the parity bounds of the kernel tests.
+
+Tolerances (SURVEY.md section 8c):
+  ids / counts / cell hashing : exact
+  SDF                         : |d| <= 1e-5 * max(|ref|, sdf_scale)
+  d sdf / d x                 : 1e-4 relative to max(|ref|, typical gradient scale)
+  feature / decoder grads     : 1e-4 relative (float atomics reorder the sums)
+  post-Adam parameters        : 1e-5 abs, a small fraction of near-zero-gradient outliers allowed
+"""
+import inspect
 import os
 
 import numpy as np
@@ -7,7 +16,86 @@ import torch
 from oracle import pin_oracle as po
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-PARITY_SLACK = []  # filled by tests/test_cuda_parity.py::assert_rel_close, reported by tests/conftest.py
+PARITY_SLACK = []  # filled by assert_rel_close, reported by tests/conftest.py
+
+
+# ---------------------------------------------------------------------------
+# parity bounds
+# ---------------------------------------------------------------------------
+def assert_sdf_close(got, ref, scale, tol=1e-5):
+    got, ref = np.asarray(got, np.float64), np.asarray(ref, np.float64)
+    bound = tol * np.maximum(np.abs(ref), scale)
+    bad = np.abs(got - ref) > bound
+    assert not bad.any(), f"{bad.sum()} / {bad.size} sdf values differ; max err {np.abs(got - ref).max():.3e}"
+
+
+def assert_rel_close(got, ref, tol, floor, ref64=None, kink_rows=0):
+    """|got - ref| <= tol * max(|ref|, floor).  When the fp64 evaluation of the same algorithm is given, the
+    fp32 reference's own rounding error |ref - ref64| is added to the bound (x4): a kernel only has to be
+    as close to the fp64 truth as the fp32 reference is (SURVEY.md section 8c, "higher-precision oracle").
+
+    `kink_rows`: derivatives of a ReLU network are discontinuous where a hidden pre-activation crosses zero; any
+    reordering of the fp32 sums (cuBLAS vs MKL vs this kernel) flips the sign of pre-activations that lie within
+    rounding of zero (~1e-6 of all activations), which changes that row's gradient by a finite amount.  Up to
+    `kink_rows` rows may therefore miss the bound, with their error still limited to 10 % of the largest value."""
+    got, ref = np.asarray(got, np.float64), np.asarray(ref, np.float64)
+    tight = tol * np.maximum(np.abs(ref), floor)
+    bound = tight
+    if ref64 is not None:
+        bound = bound + 4.0 * np.abs(ref - np.asarray(ref64, np.float64))
+    err = np.abs(got - ref)
+    bad = err > bound
+    # how much of the allowance was actually used (reported at the end of the session, tests/conftest.py)
+    rows_bad = int(bad.reshape(bad.shape[0], -1).any(axis=1).sum()) if bad.ndim else int(bad)
+    PARITY_SLACK.append({
+        "test": next((f.function for f in inspect.stack() if f.function.startswith("test_")), "?"),
+        "elements": int(err.size), "tol": tol, "over_tight_bound": int((err > tight).sum()),
+        "needed_fp64_slack": int(((err > tight) & ~bad).sum()), "kink_rows_used": rows_bad if kink_rows else 0,
+        "kink_rows_allowed": int(kink_rows), "max_err_over_tight_bound": float((err / np.maximum(tight, 1e-300)).max())})
+    if kink_rows and bad.any():
+        rows = bad.reshape(bad.shape[0], -1).any(axis=1)
+        assert rows.sum() <= kink_rows, f"{int(rows.sum())} rows miss the bound (allowed {kink_rows}); max err {err.max():.3e}"
+        assert err.max() <= 0.1 * np.abs(ref).max(), f"kink-row error {err.max():.3e} too large"
+        return
+    assert not bad.any(), f"max err {err.max():.3e} (bound {bound.min():.3e}); {int(bad.sum())} bad"
+
+
+def assert_decoder_grad_close(got, ref, ref64):
+    """Decoder gradients are sums over ALL sample rows, so one ReLU kink flip (see assert_rel_close) shifts every
+    entry a little instead of one row a lot: tight bound first, else the kink-level bound 5e-3 of the largest
+    entry on the maximum and 1e-3 on the median (a wrong kernel is off by O(1))."""
+    got, ref = np.asarray(got, np.float64), np.asarray(ref, np.float64)
+    scale = np.abs(ref).max()
+    try:
+        assert_rel_close(got, ref, 1e-4, scale * 5e-2, ref64)
+    except AssertionError:
+        err = np.abs(got - ref)
+        assert err.max() <= 5e-3 * scale and np.median(err) <= 1e-3 * scale, \
+            f"decoder gradient: max err {err.max():.3e}, median {np.median(err):.3e}, scale {scale:.3e}"
+
+
+def assert_close_frac(a, b, atol=1e-5, max_bad_frac=5e-3, max_abs=4e-2):
+    """Parameters after a few Adam steps: Adam's eps 1e-15 turns near-zero gradients into +-lr steps whose sign
+    follows the summation order, so a small fraction of entries may differ by up to a few lr."""
+    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
+    bad = np.abs(a - b) > atol + 1e-5 * np.abs(b)
+    assert bad.mean() <= max_bad_frac, f"{bad.sum()} / {bad.size} differ, max {np.abs(a - b).max():.2e}"
+    assert np.abs(a - b).max() <= max_abs
+
+
+def oracle64(m, dec, q, k, wf, ref32, **kw):
+    """fp64 run of the oracle; rows whose neighbour set differs from the fp32 run (a query within one ulp
+    of a voxel boundary) fall back to the fp32 values."""
+    kw = {a: (b.double() if isinstance(b, po.DecoderParams) else b) for a, b in kw.items()}
+    r64 = po.query_sdf(m.double(), dec.double(), q.double(), k, wf, **kw)
+    same = (r64["nn_count"] == ref32["nn_count"]).numpy()
+    out = {}
+    for name in ("sdf", "grad", "sdf_std", "color", "color_grad"):
+        if name in r64 and name in ref32:
+            a, b = r64[name].numpy(), np.asarray(ref32[name], np.float64)
+            sel = same.reshape((-1,) + (1,) * (a.ndim - 1))
+            out[name] = np.where(sel, a, b)
+    return out
 
 
 def load_npz(name):
@@ -118,6 +206,52 @@ def queries_near(m, n, seed, sigma=0.15):
 
 
 # ---------------------------------------------------------------------------
+# K2 cases: the instantiation each one must launch (read by the coverage ledger of tests/test_query_paths.py)
+# ---------------------------------------------------------------------------
+def train_bwd_kernel_name(F, L, aligned=True):
+    """The K2 kernel pinb200_train_backward launches for a 64-wide decoder with L hidden layers on F features
+    (dispatch_train_mma in train_mma.cuh: 1-2 layers on a 16-byte aligned feature table; else the SIMT kernel by padded
+    input width in train.cu)."""
+    if L <= 2 and aligned:
+        return f"train_bwd_mma_kernel<{F}, {L}>"
+    return f"train_bwd_kernel<64, {next(dp for dp in (12, 20, 36, 68) if F + 3 <= dp)}>"
+
+
+# (F, K, L, weighted_first, out_dim, after_pgo, leaky, bias, aligned) of
+# test_cuda_parity.py::test_train_backward_vs_autograd_synthetic.  aligned=False: the feature table starts 4 bytes
+# past a 16-byte boundary.  The SIMT kernel's shared memory fits 3 hidden layers only for F <= 8, so its wider
+# instantiations run on 1-2 layer decoders over such tables.
+TRAIN_BWD_CASES = [
+    (8, 6, 1, False, 1, False, False, True, True), (8, 6, 1, True, 1, False, False, True, True),
+    (4, 4, 1, True, 1, True, False, True, True), (16, 5, 2, False, 1, False, False, True, True),
+    (32, 8, 2, True, 1, False, False, True, True), (64, 8, 1, False, 1, True, False, True, True),
+    (64, 3, 2, True, 3, False, False, True, True), (8, 6, 2, False, 3, False, False, True, True),
+    (4, 6, 3, True, 1, False, False, True, True),
+    (16, 4, 1, True, 1, False, True, False, True), (32, 7, 1, False, 1, False, False, False, True),
+    (4, 5, 2, False, 3, True, True, True, True), (8, 6, 2, True, 1, False, False, False, True),
+    (32, 8, 2, False, 3, False, True, False, True), (8, 5, 3, False, 1, False, True, False, True),
+    (16, 6, 2, False, 1, False, True, True, False), (32, 8, 1, True, 1, True, False, False, False),
+    (64, 3, 2, False, 3, False, False, True, False),
+]
+
+
+def kernels_run(fn, tries=3):
+    """fn() under torch.profiler with CUDA activity: (its result, the demangled names of the kernels it launched).
+    Now and then the profiler loses a whole activity buffer, and the trace holds no kernel at all; fn() then runs
+    again (up to `tries` times), so it must be repeatable."""
+    from torch.profiler import ProfilerActivity, profile
+
+    for _ in range(tries):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            out = fn()
+            torch.cuda.synchronize()
+        names = {e.key for e in prof.key_averages()}
+        if any("pinb::" in k for k in names):
+            break
+    return out, names
+
+
+# ---------------------------------------------------------------------------
 # CUDA-side helpers (only used by -m gpu tests, smoke and bench)
 # ---------------------------------------------------------------------------
 def map_handle_from_oracle(m, query_locally=True, device="cuda", color=True):
@@ -151,20 +285,24 @@ def map_handle_from_oracle(m, query_locally=True, device="cuda", color=True):
     )
 
 
-def decoder_handle_from_oracle(dec, device="cuda", sigmoid_out=False):
+def decoder_handle_from_oracle(dec, device="cuda", sigmoid_out=False, bias=True):
+    """`bias=False`: a decoder without biases (mlp_bias_on False) -- the handle passes NULL bias pointers; the oracle
+    decoder (po.make_decoder(..., bias=False)) keeps zero biases, which gives the same forward pass."""
     from pin_slam_b200 import ops
 
     dev = torch.device(device)
     ws = [w.detach().contiguous().to(dev) for w, _ in dec.hidden]
-    bs = [b.detach().contiguous().to(dev) for _, b in dec.hidden]
-    return ops.DecoderHandle(ws, bs, dec.out[0].detach().contiguous().to(dev), dec.out[1].detach().contiguous().to(dev),
+    bs = [b.detach().contiguous().to(dev) if bias else None for _, b in dec.hidden]
+    bo = dec.out[1].detach().contiguous().to(dev) if bias else None
+    return ops.DecoderHandle(ws, bs, dec.out[0].detach().contiguous().to(dev), bo,
                              out_scale=1.0 if sigmoid_out else dec.sdf_scale, leaky=dec.leaky, sigmoid_out=sigmoid_out)
 
 
-def flat_decoder_params(dec):
-    """[w0|b0|w1|b1|...|w_out|b_out] -- the layout pinb200_train_backward / adam use."""
+def flat_decoder_params(dec, bias=True):
+    """[w0|b0|w1|b1|...|w_out|b_out] -- the layout pinb200_train_backward / adam use; `bias=False` leaves the bias
+    blocks out, as Decoder.flat_parameters() does for a decoder without biases."""
     parts = []
     for w, b in dec.hidden:
-        parts += [w.detach().reshape(-1), b.detach().reshape(-1)]
-    parts += [dec.out[0].detach().reshape(-1), dec.out[1].detach().reshape(-1)]
+        parts += [w.detach().reshape(-1)] + ([b.detach().reshape(-1)] if bias else [])
+    parts += [dec.out[0].detach().reshape(-1)] + ([dec.out[1].detach().reshape(-1)] if bias else [])
     return torch.cat(parts)

@@ -1,21 +1,15 @@
 """GPU parity tests: every CUDA entry point (through the C ABI) against the CPU
 oracle on the same seeded inputs, and against the golden fixtures recorded from
-the unmodified reference.
-
-Tolerances (SURVEY.md section 8c):
-  ids / counts / cell hashing : exact
-  SDF                         : |d| <= 1e-5 * max(|ref|, sdf_scale)
-  d sdf / d x                 : 1e-4 relative to max(|ref|, typical gradient scale)
-  feature / decoder grads     : 1e-4 relative (float atomics reorder the sums)
-  post-Adam parameters        : 1e-5 abs, a small fraction of near-zero-gradient outliers allowed
-"""
+the unmodified reference.  The tolerances are those of tests/helpers.py."""
 import numpy as np
 import pytest
 import torch
 
 from oracle import pin_oracle as po
-from tests.helpers import (decoder_from_fixture, decoder_handle_from_oracle, flat_decoder_params, load_npz,
-                           map_from_fixture, map_handle_from_oracle, queries_near, synthetic_map, t)
+from tests.helpers import (TRAIN_BWD_CASES, assert_close_frac, assert_decoder_grad_close, assert_rel_close,
+                           assert_sdf_close, decoder_from_fixture, decoder_handle_from_oracle, flat_decoder_params, kernels_run,
+                           load_npz, map_from_fixture, map_handle_from_oracle, oracle64, queries_near, synthetic_map, t,
+                           train_bwd_kernel_name)
 
 pytestmark = pytest.mark.gpu
 
@@ -28,77 +22,6 @@ def ops():
     from pin_slam_b200 import ops as _ops
 
     return _ops
-
-
-def assert_sdf_close(got, ref, scale, tol=1e-5):
-    got, ref = np.asarray(got, np.float64), np.asarray(ref, np.float64)
-    bound = tol * np.maximum(np.abs(ref), scale)
-    bad = np.abs(got - ref) > bound
-    assert not bad.any(), f"{bad.sum()} / {bad.size} sdf values differ; max err {np.abs(got - ref).max():.3e}"
-
-
-def assert_rel_close(got, ref, tol, floor, ref64=None, kink_rows=0):
-    """|got - ref| <= tol * max(|ref|, floor).  When the fp64 evaluation of the same algorithm is given, the
-    fp32 reference's own rounding error |ref - ref64| is added to the bound (x4): a kernel only has to be
-    as close to the fp64 truth as the fp32 reference is (SURVEY.md section 8c, "higher-precision oracle").
-
-    `kink_rows`: derivatives of a ReLU network are discontinuous where a hidden pre-activation crosses zero; any
-    reordering of the fp32 sums (cuBLAS vs MKL vs this kernel) flips the sign of pre-activations that lie within
-    rounding of zero (~1e-6 of all activations), which changes that row's gradient by a finite amount.  Up to
-    `kink_rows` rows may therefore miss the bound, with their error still limited to 10 % of the largest value."""
-    got, ref = np.asarray(got, np.float64), np.asarray(ref, np.float64)
-    tight = tol * np.maximum(np.abs(ref), floor)
-    bound = tight
-    if ref64 is not None:
-        bound = bound + 4.0 * np.abs(ref - np.asarray(ref64, np.float64))
-    err = np.abs(got - ref)
-    bad = err > bound
-    # how much of the allowance was actually used (reported at the end of the session, tests/conftest.py)
-    import inspect
-
-    from tests import helpers
-
-    rows_bad = int(bad.reshape(bad.shape[0], -1).any(axis=1).sum()) if bad.ndim else int(bad)
-    helpers.PARITY_SLACK.append({
-        "test": next((f.function for f in inspect.stack() if f.function.startswith("test_")), "?"),
-        "elements": int(err.size), "tol": tol, "over_tight_bound": int((err > tight).sum()),
-        "needed_fp64_slack": int(((err > tight) & ~bad).sum()), "kink_rows_used": rows_bad if kink_rows else 0,
-        "kink_rows_allowed": int(kink_rows), "max_err_over_tight_bound": float((err / np.maximum(tight, 1e-300)).max())})
-    if kink_rows and bad.any():
-        rows = bad.reshape(bad.shape[0], -1).any(axis=1)
-        assert rows.sum() <= kink_rows, f"{int(rows.sum())} rows miss the bound (allowed {kink_rows}); max err {err.max():.3e}"
-        assert err.max() <= 0.1 * np.abs(ref).max(), f"kink-row error {err.max():.3e} too large"
-        return
-    assert not bad.any(), f"max err {err.max():.3e} (bound {bound.min():.3e}); {int(bad.sum())} bad"
-
-
-def assert_decoder_grad_close(got, ref, ref64):
-    """Decoder gradients are sums over ALL sample rows, so one ReLU kink flip (see assert_rel_close) shifts every
-    entry a little instead of one row a lot: tight bound first, else the kink-level bound 5e-3 of the largest
-    entry on the maximum and 1e-3 on the median (a wrong kernel is off by O(1))."""
-    got, ref = np.asarray(got, np.float64), np.asarray(ref, np.float64)
-    scale = np.abs(ref).max()
-    try:
-        assert_rel_close(got, ref, 1e-4, scale * 5e-2, ref64)
-    except AssertionError:
-        err = np.abs(got - ref)
-        assert err.max() <= 5e-3 * scale and np.median(err) <= 1e-3 * scale, \
-            f"decoder gradient: max err {err.max():.3e}, median {np.median(err):.3e}, scale {scale:.3e}"
-
-
-def oracle64(m, dec, q, k, wf, ref32, **kw):
-    """fp64 run of the oracle; rows whose neighbour set differs from the fp32 run (a query within one ulp
-    of a voxel boundary) fall back to the fp32 values."""
-    kw = {a: (b.double() if isinstance(b, po.DecoderParams) else b) for a, b in kw.items()}
-    r64 = po.query_sdf(m.double(), dec.double(), q.double(), k, wf, **kw)
-    same = (r64["nn_count"] == ref32["nn_count"]).numpy()
-    out = {}
-    for name in ("sdf", "grad", "sdf_std", "color", "color_grad"):
-        if name in r64 and name in ref32:
-            a, b = r64[name].numpy(), np.asarray(ref32[name], np.float64)
-            sel = same.reshape((-1,) + (1,) * (a.ndim - 1))
-            out[name] = np.where(sel, a, b)
-    return out
 
 
 # --------------------------------------------------------------------------------------
@@ -452,18 +375,24 @@ def test_train_backward_matches_autograd(name):
     assert np.array_equal(mh.keep["ts_update"].cpu().numpy(), m.local_point_ts_update.numpy())
 
 
-@pytest.mark.parametrize("F,K,L,wf,oc,pgo", [(8, 6, 1, False, 1, False), (8, 6, 1, True, 1, False),
-                                               (4, 4, 1, True, 1, True), (16, 5, 2, False, 1, False),
-                                               (32, 8, 2, True, 1, False), (64, 8, 1, False, 1, True),
-                                               (64, 3, 2, True, 3, False), (8, 6, 2, False, 3, False),
-                                               (4, 6, 3, True, 1, False)])
-def test_train_backward_vs_autograd_synthetic(F, K, L, wf, oc, pgo):
-    """K2 on every tensor-core instantiation (1-2 hidden layers) and the SIMT fallback (3 layers): gradients of
-    sum(out * dl) w.r.t. the feature table and the decoder, against fp32/fp64 autograd through the oracle."""
+def _train_case_id(c):
+    F, K, L, wf, oc, pgo, leaky, bias, aligned = c
+    return (f"{F}-{K}-{L}-{wf}-{oc}-{pgo}" + ("-leaky" if leaky else "") + ("" if bias else "-nobias")
+            + ("" if aligned else "-unaligned"))
+
+
+@pytest.mark.parametrize("F,K,L,wf,oc,pgo,leaky,bias,aligned", TRAIN_BWD_CASES,
+                         ids=[_train_case_id(c) for c in TRAIN_BWD_CASES])
+def test_train_backward_vs_autograd_synthetic(F, K, L, wf, oc, pgo, leaky, bias, aligned):
+    """K2 on every tensor-core instantiation (1-2 hidden layers, aligned feature table) and every SIMT instantiation
+    (3 layers, or a feature table off the 16-byte grid), ReLU and leaky ReLU, with and without biases: gradients of
+    sum(out * dl) w.r.t. the feature table and the decoder, against fp32/fp64 autograd through the oracle.  grad_dec
+    is followed by a sentinel tail the kernel must not touch."""
     m = synthetic_map(n_surface=30000, seed=F + K + L, resolution=0.4, buffer_size=200003, feature_dim=F,
                       after_pgo=pgo, local_radius=14.0, diff_td=3.0)
     sig = oc > 1
-    dec = po.make_decoder(F + 3, 64, L, oc, 0.044, seed=L)
+    dec = po.make_decoder(F + 3, 64, L, oc, 0.044, seed=L, bias=bias)
+    dec.leaky = leaky
     n = 7001  # not a multiple of the tile size
     q = queries_near(m, n, seed=9)
     q[:5] = torch.tensor([300.0, -200.0, 50.0])  # no neighbours
@@ -480,23 +409,37 @@ def test_train_backward_vs_autograd_synthetic(F, K, L, wf, oc, pgo):
             o = po.decoder_color(dd, flat) if sig else po.decoder_sdf(dd, flat).unsqueeze(1)
             out = (o.view(qq.shape[0], K, oc) * w).sum(1)
         (out * dll).sum().backward()
-        return mm.local_geo_features.grad, torch.cat([p.grad.reshape(-1) for p in dd.tensors()])
+        params = dd.tensors() if bias else [w for w, _ in dd.hidden] + [dd.out[0]]  # a bias-free decoder: weights only
+        return mm.local_geo_features.grad, torch.cat([p.grad.reshape(-1) for p in params])
 
     gf_ref, gd_ref = reference(m.clone(), dec.clone(), q, dl)
     gf64, gd64 = reference(m.clone().double(), dec.double(), q.double(), dl.double())
     mh = map_handle_from_oracle(m, True)
-    dh = decoder_handle_from_oracle(dec, sigmoid_out=sig)
+    dh = decoder_handle_from_oracle(dec, sigmoid_out=sig, bias=bias)
     idx, _, w, _ = ops().knn_search(mh, q.cuda(), K)[:4]
+    feat = mh.keep["geo_feat"]
+    if not aligned:
+        feat = torch.empty(feat.numel() + 1, device="cuda")[1:].view_as(feat).copy_(feat)
     gfeat = torch.zeros_like(mh.keep["geo_feat"])
-    gdec = torch.zeros(dh.param_count(), device="cuda")
-    ops().train_backward(mh, dh, mh.keep["geo_feat"], q.cuda(), idx, w, dl.cuda(), wf, gfeat, gdec)
+    n_par = gd_ref.numel()
+    buf = torch.full((n_par + 256,), 12345.0, device="cuda")  # the flat gradient, then a sentinel tail
+    gdec = buf[:n_par].zero_()
+    _, names = kernels_run(lambda: ops().train_backward(mh, dh, feat, q.cuda(), idx, w, dl.cuda(), wf,
+                                                        torch.zeros_like(gfeat), torch.zeros_like(gdec)))
+    assert any(train_bwd_kernel_name(F, L, aligned) in k for k in names), names
+    ops().train_backward(mh, dh, feat, q.cuda(), idx, w, dl.cuda(), wf, gfeat, gdec)
+    assert bool((buf[n_par:] == 12345.0).all()), "train_backward wrote past the end of grad_dec"
     # 3xTF32 keeps ~21 mantissa bits per product: bound = 1e-4 relative with a floor of 5 % of the largest entry
     # (5e-6 of the gradient scale), plus the fp32 reference's own distance to fp64; ReLU kink rows as documented
     assert_rel_close(gfeat.cpu(), gf_ref, 1e-4, float(gf_ref.abs().max()) * 5e-2, gf64, kink_rows=8)
     assert_decoder_grad_close(gdec.cpu(), gd_ref, gd64)
     # second call accumulates
-    ops().train_backward(mh, dh, mh.keep["geo_feat"], q.cuda(), idx, w, dl.cuda(), wf, gfeat, gdec)
+    ops().train_backward(mh, dh, feat, q.cuda(), idx, w, dl.cuda(), wf, gfeat, gdec)
     assert_decoder_grad_close(0.5 * gdec.cpu(), gd_ref, gd64)
+    assert bool((buf[n_par:] == 12345.0).all()), "train_backward wrote past the end of grad_dec"
+    # a flat gradient of any other length is refused before the launch
+    with pytest.raises(RuntimeError):
+        ops().train_backward(mh, dh, feat, q.cuda(), idx, w, dl.cuda(), wf, gfeat, buf)
 
 
 def test_adam_matches_torch():
@@ -577,18 +520,11 @@ def test_three_mapping_iterations_match_reference(name):
         ops().adam_step(flat, gdec, md, vd, lr, 0.9, 0.99, adam_eps, 0.0, it + 1)
         ops().adam_step(feat, gfeat, mf, vf, lr, 0.9, 0.99, adam_eps, wd, it + 1)
     torch.cuda.synchronize()
-
-    def close_frac(a, b, atol=1e-5, max_bad_frac=5e-3, max_abs=4e-2):
-        a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-        bad = np.abs(a - b) > atol + 1e-5 * np.abs(b)
-        assert bad.mean() <= max_bad_frac, f"{bad.sum()} / {bad.size} differ, max {np.abs(a - b).max():.2e}"
-        assert np.abs(a - b).max() <= max_abs
-
-    close_frac(feat.cpu().numpy(), fx["after.local_geo_features"])
-    close_frac(flat.cpu().numpy(), _ref_flat(fx, "sdf_mlp", dec))
+    assert_close_frac(feat.cpu().numpy(), fx["after.local_geo_features"])
+    assert_close_frac(flat.cpu().numpy(), _ref_flat(fx, "sdf_mlp", dec))
     if color:
-        close_frac(cfeat.cpu().numpy(), fx["after.local_color_features"])
-        close_frac(cflat.cpu().numpy(), _ref_flat(fx, "color_mlp", cdec))
+        assert_close_frac(cfeat.cpu().numpy(), fx["after.local_color_features"])
+        assert_close_frac(cflat.cpu().numpy(), _ref_flat(fx, "color_mlp", cdec))
     np.testing.assert_allclose(mh.keep["certainty"].cpu().numpy(), fx["after.local_point_certainties"], rtol=1e-4,
                                atol=1e-4)
     assert np.array_equal(mh.keep["ts_update"].cpu().numpy(), fx["after.local_point_ts_update"])

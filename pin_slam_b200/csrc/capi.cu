@@ -2,6 +2,9 @@
 #include <stdarg.h>
 #include <string.h>
 
+#include <mutex>
+#include <vector>
+
 #include "common.cuh"
 
 namespace pinb {
@@ -34,6 +37,40 @@ int sm_count() {
     if (cached <= 0) cached = 132;
   }
   return cached;
+}
+
+int prepare_kernel(const void* fn, const char* what, size_t smem_bytes, int threads, int* occ) {
+  struct Prepared {
+    int dev;
+    const void* fn;
+    size_t smem;
+    int occ;  // 0: not asked for yet
+  };
+  static std::mutex mu;
+  static std::vector<Prepared> done;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  std::lock_guard<std::mutex> lk(mu);
+  Prepared* k = nullptr;
+  for (Prepared& c : done)
+    if (c.dev == dev && c.fn == fn && c.smem == smem_bytes) k = &c;
+  if (!k) {
+    const cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess) {
+      set_error("cudaFuncSetAttribute(%s): %s", what, cudaGetErrorString(e));
+      return PINB200_ERR_CUDA;
+    }
+    done.push_back({dev, fn, smem_bytes, 0});
+    k = &done.back();
+  }
+  if (occ) {
+    if (k->occ == 0) {
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k->occ, fn, threads, smem_bytes);
+      if (k->occ < 1) k->occ = 1;
+    }
+    *occ = k->occ;
+  }
+  return PINB200_OK;
 }
 
 }  // namespace pinb

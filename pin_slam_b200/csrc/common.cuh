@@ -24,6 +24,13 @@ int check_launch(const char* what);
 int sm_count();
 int nccl_allreduce_sum(void* comm, float* buf, int64_t count, cudaStream_t stream);  // collective.cu
 
+// Lets kernel `fn` use up to 227 KB of dynamic shared memory and, with `occ`, stores its resident CTAs per SM (>= 1)
+// at `threads` threads and `smem_bytes` of dynamic shared memory.  The attribute and occupancy calls cost a few
+// microseconds each, so they run once per (device, kernel, smem_bytes).  Returns PINB200_OK or PINB200_ERR_CUDA.
+int prepare_kernel(const void* fn, const char* what, size_t smem_bytes, int threads = 0, int* occ = nullptr);
+
+__host__ __device__ inline int align4(int x) { return (x + 3) & ~3; }
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);

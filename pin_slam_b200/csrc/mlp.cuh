@@ -23,8 +23,6 @@ struct DecSmem {  // offsets in floats from the dynamic-smem base (all multiples
   int end;                            // first free float
 };
 
-__host__ __device__ inline int align4(int x) { return (x + 3) & ~3; }
-
 inline DecSmem plan_decoder_smem(const pinb200_decoder_view& d, int DP, bool with_bwd_layout, int start) {
   DecSmem s{};
   int o = align4(start);

@@ -1,41 +1,64 @@
-// Warp-level tensor-core decoder for the per-warp 32-row tiles of K1.
+// Warp-level tensor-core decoder building blocks of the query kernel (K1, query_kernel) and the tensor-core training
+// backward (K2, train_bwd_mma_kernel).
 //
 // The decoder is a chain of [32 x K] x [K x 64] contractions per warp tile, issued as mma.sync.m16n8k8 TF32
 // tensor-core instructions with the 3xTF32 split  a*b ~= a_hi*b_hi + a_lo*b_hi + a_hi*b_lo  (a_hi = a with the low
 // 13 mantissa bits cleared, a_lo = a - a_hi exactly), which keeps ~21 mantissa bits: the SDF stays within the 1e-5
 // parity bound of the fp32 reference.  Weights are split once per CTA when they are staged into shared memory.
 //
-// Register chaining (round 2): the k index of a contraction may be permuted freely as long as A and B agree.  With
+// Register chaining (K1): the k index of a contraction may be permuted freely as long as A and B agree.  With
 // the permutation  slot t <-> unit 8kk+2t,  slot t+4 <-> unit 8kk+2t+1  of every k-step the C fragments of one layer
 // ARE the A fragments of the next one (c0,c2,c1,c3 -> a0,a1,a2,a3), so the activations never leave the register
-// file between layers (round 1 stored every layer's output to a 32x68 shared-memory tile and re-loaded it), and the
-// two B values of a lane become adjacent in the nn.Linear row: one LDS.64 per (hi | lo) fragment instead of two
-// LDS.32.  Leading dimensions == 8 (mod 32) make those 64-bit fragment loads bank-conflict free.
+// file between layers, and the two B values of a lane become adjacent in the nn.Linear row: one LDS.64 per (hi | lo)
+// fragment instead of two LDS.32.  Leading dimensions == 8 (mod 32) make those 64-bit fragment loads bank-conflict
+// free.  K2 keeps its activations in row-major shared-memory tiles (it needs them again for the weight gradients)
+// and multiplies them with warp_gemm_3xtf32, whose scalar fragment loads are conflict free with leading dimensions
+// == 4 (mod 32).
 //
 // (wgmma needs 64-row warpgroup tiles and a warpgroup-wide issue / wait choreography; with independent 32-row warp
 // tiles the warp-synchronous mma.sync form is the natural fit.  DESIGN.md section 7 discusses the trade-off.)
 #pragma once
-#include "mlp_mma.cuh"
+#include "common.cuh"
 
 namespace pinb {
 
-struct ChainDecSmem {  // float offsets from the dynamic-smem base
-  int whi[PINB200_MAX_HIDDEN_LAYERS];  // [H][ldw_l]  tf32 "hi" part, torch layout, zero padded
-  int wlo[PINB200_MAX_HIDDEN_LAYERS];  // [H][ldw_l]  tf32 "lo" part
-  int b[PINB200_MAX_HIDDEN_LAYERS];    // [H]
-  int ldw[PINB200_MAX_HIDDEN_LAYERS];  // == 8 (mod 32), >= padded fan-in
-  int wout, bout, end;
-};
+constexpr uint32_t TF32_MASK = 0xffffe000u;
+
+// decoder input width (FT features + 3 position components) padded to the MMA k-step
+__host__ __device__ constexpr int dec_in_pad(int FT) { return (FT + 3 + 7) / 8 * 8; }
 
 // smallest leading dimension >= x that is == 8 (mod 32): conflict-free 64-bit fragment loads
 __host__ __device__ constexpr int ld8mod32(int x) { return x <= 8 ? 8 : ((x - 8 + 31) / 32) * 32 + 8; }
 
-inline ChainDecSmem plan_chain_decoder_smem(const pinb200_decoder_view& d, int KP0, int start) {
-  ChainDecSmem s{};
-  int o = align4i(start);
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+
+__device__ __forceinline__ void split_tf32(float v, uint32_t& hi, uint32_t& lo) {
+  hi = __float_as_uint(v) & TF32_MASK;
+  lo = __float_as_uint(v - __uint_as_float(hi)) & TF32_MASK;
+}
+
+struct WarpDecSmem {  // float offsets from the dynamic-smem base
+  int whi[PINB200_MAX_HIDDEN_LAYERS];  // [H][ldw_l]  tf32 "hi" part, torch layout, zero padded
+  int wlo[PINB200_MAX_HIDDEN_LAYERS];  // [H][ldw_l]  tf32 "lo" part
+  int b[PINB200_MAX_HIDDEN_LAYERS];    // [H]
+  int ldw[PINB200_MAX_HIDDEN_LAYERS];  // ld(padded fan-in of layer l)
+  int wout, bout, end;
+};
+
+// KP0: padded fan-in of layer 0; ld(fan_in) -> leading dimension of a weight matrix (the kernel's fragment loads
+// decide which one is bank-conflict free)
+template <class Ld>
+inline WarpDecSmem plan_warp_decoder_smem(const pinb200_decoder_view& d, int KP0, int start, Ld ld) {
+  WarpDecSmem s{};
+  int o = align4(start);
   const int H = d.hidden_dim;
   for (int l = 0; l < d.n_hidden; ++l) {
-    s.ldw[l] = ld8mod32(l == 0 ? KP0 : H);
+    s.ldw[l] = ld(l == 0 ? KP0 : H);
     s.whi[l] = o;
     o += H * s.ldw[l];
     s.wlo[l] = o;
@@ -46,12 +69,12 @@ inline ChainDecSmem plan_chain_decoder_smem(const pinb200_decoder_view& d, int K
   s.wout = o;
   o += d.out_dim * H;
   s.bout = o;
-  o += align4i(d.out_dim);
+  o += align4(d.out_dim);
   s.end = o;
   return s;
 }
 
-__device__ __forceinline__ void stage_chain_decoder(const pinb200_decoder_view& d, const ChainDecSmem& s, float* smem) {
+__device__ __forceinline__ void stage_warp_decoder(const pinb200_decoder_view& d, const WarpDecSmem& s, float* smem) {
   const int H = d.hidden_dim, nt = blockDim.x, tid = threadIdx.x;
   for (int l = 0; l < d.n_hidden; ++l) {
     const int in = l == 0 ? d.in_dim : H, ldw = s.ldw[l];
@@ -71,7 +94,7 @@ __device__ __forceinline__ void stage_chain_decoder(const pinb200_decoder_view& 
   float* wo = smem + s.wout;
   for (int e = tid; e < d.out_dim * H; e += nt) wo[e] = __ldg(d.w_out + e);
   float* bo = smem + s.bout;
-  for (int e = tid; e < align4i(d.out_dim); e += nt) bo[e] = (d.b_out && e < d.out_dim) ? __ldg(d.b_out + e) : 0.f;
+  for (int e = tid; e < align4(d.out_dim); e += nt) bo[e] = (d.b_out && e < d.out_dim) ? __ldg(d.b_out + e) : 0.f;
 }
 
 template <int NT>
@@ -82,6 +105,71 @@ __device__ __forceinline__ void zero_frags(float (&acc)[2][NT][4]) {
     for (int nt = 0; nt < NT; ++nt)
 #pragma unroll
       for (int c = 0; c < 4; ++c) acc[mt][nt][c] = 0.f;
+}
+
+// C-fragment coordinates of element c of block (mt, nt) for this lane
+__device__ __forceinline__ int frag_row(int mt, int c, int lane) { return mt * 16 + (lane >> 2) + 8 * (c >> 1); }
+__device__ __forceinline__ int frag_col(int nt, int c, int lane) { return nt * 8 + 2 * (lane & 3) + (c & 1); }
+
+// x[row][col] = acc (float2 stores); caller brackets with __syncwarp()
+template <int NT, int LDX>
+__device__ __forceinline__ void store_frags(float* __restrict__ x, const float (&acc)[2][NT][4], int lane) {
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float2 v = make_float2(acc[mt][nt][2 * h], acc[mt][nt][2 * h + 1]);
+        *reinterpret_cast<float2*>(x + frag_row(mt, 2 * h, lane) * LDX + frag_col(nt, 0, lane)) = v;
+      }
+    }
+}
+
+// K2: acc[mt][nt] (16x8 C fragments, mt < 2 row blocks, nt < NT column blocks) = X[32 x 8*KT] * B, X row-major in
+// shared memory (leading dimension LDX == 4 mod 32), k in natural order
+//   BWD == false: B[k][n] = W[n][k]   (forward layer:  h = x W^T)
+//   BWD == true : B[k][n] = W[k][n]   (backward layer: g_in = g_out W)
+template <int KT, int NT, bool BWD, int LDX>
+__device__ __forceinline__ void warp_gemm_3xtf32(float (&acc)[2][NT][4], const float* __restrict__ x,
+                                                 const float* __restrict__ whi, const float* __restrict__ wlo, int ldw,
+                                                 int lane) {
+  const int g = lane >> 2, t = lane & 3;
+  zero_frags<NT>(acc);
+#pragma unroll 1
+  for (int kk = 0; kk < KT; ++kk) {
+    uint32_t ah[2][4], al[2][4];
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt) {
+      const float* xr = x + (mt * 16 + g) * LDX + kk * 8 + t;
+      split_tf32(xr[0], ah[mt][0], al[mt][0]);
+      split_tf32(xr[8 * LDX], ah[mt][1], al[mt][1]);
+      split_tf32(xr[4], ah[mt][2], al[mt][2]);
+      split_tf32(xr[8 * LDX + 4], ah[mt][3], al[mt][3]);
+    }
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt) {
+      int o0, o1;
+      if (!BWD) {
+        o0 = (nt * 8 + g) * ldw + kk * 8 + t;
+        o1 = o0 + 4;
+      } else {
+        o0 = (kk * 8 + t) * ldw + nt * 8 + g;
+        o1 = o0 + 4 * ldw;
+      }
+      uint32_t bh[2], bl[2];
+      bh[0] = __float_as_uint(whi[o0]);
+      bh[1] = __float_as_uint(whi[o1]);
+      bl[0] = __float_as_uint(wlo[o0]);
+      bl[1] = __float_as_uint(wlo[o1]);
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt) {
+        mma_tf32(acc[mt][nt], al[mt], bh);  // small terms first
+        mma_tf32(acc[mt][nt], ah[mt], bl);
+        mma_tf32(acc[mt][nt], ah[mt], bh);
+      }
+    }
+  }
 }
 
 // one k-step of the forward contraction against W[n_out][k_in] (nn.Linear layout): B pairs are adjacent floats
@@ -189,6 +277,7 @@ __device__ __forceinline__ void gemm_chain_bwd(float (&out)[2][NT][4], const flo
 }
 
 // bias + (leaky) ReLU in place; returns the 64-bit mask of positive pre-activations in fragment order
+// (bit mt*32 + nt*4 + c).  `bias` is 8-byte aligned.
 template <int NT>
 __device__ __forceinline__ uint64_t bias_act_chain(float (&acc)[2][NT][4], const float* __restrict__ bias, bool leaky,
                                                    int lane) {
@@ -211,6 +300,7 @@ __device__ __forceinline__ uint64_t bias_act_chain(float (&acc)[2][NT][4], const
   return (uint64_t)mk[0] | ((uint64_t)mk[1] << 32);
 }
 
+// the (leaky) ReLU derivative of a bias_act_chain mask applied to a gradient in the same fragment order
 template <int NT>
 __device__ __forceinline__ void mask_chain(float (&acc)[2][NT][4], uint64_t mk64, bool leaky) {
   const uint32_t mk[2] = {(uint32_t)mk64, (uint32_t)(mk64 >> 32)};

@@ -52,9 +52,9 @@ __global__ void __launch_bounds__(128, 4) search_kernel(const __grid_constant__ 
 template <int FT, bool WF, bool SPLIT>
 __global__ void __launch_bounds__(WPB * 32, 1) query_kernel(const __grid_constant__ QueryParams p) {
   constexpr int H = 64;
-  constexpr int KP0 = (FT + 3 + 7) / 8 * 8;  // decoder input width padded to the MMA k-step
-  constexpr int KT0 = KP0 / 8;               // k-steps of layer 0 == n-tiles of the input gradient
-  constexpr int LDX = ld8mod32(KP0);         // row-major tile leading dimension (== 8 mod 32)
+  constexpr int KP0 = dec_in_pad(FT);  // decoder input width padded to the MMA k-step
+  constexpr int KT0 = KP0 / 8;         // k-steps of layer 0 == n-tiles of the input gradient
+  constexpr int LDX = ld8mod32(KP0);   // row-major tile leading dimension (== 8 mod 32)
   constexpr int F = FT, D = FT + 3;
   extern __shared__ __align__(16) float smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -84,7 +84,7 @@ __global__ void __launch_bounds__(WPB * 32, 1) query_kernel(const __grid_constan
   float* s_dv = wsm + WL::dv;
   uint64_t* s_mask = reinterpret_cast<uint64_t*>(wsm + WL::mask);
 
-  stage_chain_decoder(p.dec, p.lay.dec, smem);
+  stage_warp_decoder(p.dec, p.lay.dec, smem);
   if (!SPLIT && !p.use_saved_knn) fill_probe_deltas(m, s_delta);
   __syncthreads();
 
@@ -533,7 +533,7 @@ static QueryLayout plan_layout(const QueryParams& p) {
   int o = 0;
   l.delta = o;
   o += align4(p.map.n_probe);
-  l.dec = plan_chain_decoder_smem(p.dec, WarpLay<FT>::KP0, o);
+  l.dec = plan_warp_decoder_smem(p.dec, WarpLay<FT>::KP0, o, ld8mod32);
   l.warp0 = align4(l.dec.end);
   int nw = (227 * 1024 / 4 - l.warp0) / WarpLay<FT>::stride;
   l.n_warps = nw > WPB ? WPB : nw;
@@ -573,29 +573,7 @@ static int launch_query(QueryParams& p, cudaStream_t stream) {
     if (per_sm < nw) nw = (int)std::max<long long>(1, per_sm);
   }
   auto kern = query_kernel<FT, WF, SPLIT>;
-  // the attribute / occupancy calls cost a few microseconds each: remember the answer per (device, kernel)
-  struct Cached {
-    int dev;
-    const void* fn;
-  };
-  static std::mutex mu;
-  static std::vector<Cached> cache;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  {
-    std::lock_guard<std::mutex> lk(mu);
-    bool known = false;
-    for (const Cached& c : cache)
-      if (c.dev == dev && c.fn == (const void*)kern) known = true;
-    if (!known) {
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-      if (e != cudaSuccess) {
-        set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-        return PINB200_ERR_CUDA;
-      }
-      cache.push_back({dev, (const void*)kern});
-    }
-  }
+  if (const int rc = prepare_kernel((const void*)kern, "query_kernel", smem_bytes)) return rc;
   const long long ctas_needed = (p.n_tiles + nw - 1) / nw;
   const int grid = (int)std::min<long long>(ctas_needed, (long long)sm_count());  // one CTA per SM (launch bounds)
   kern<<<grid, nw * 32, smem_bytes, stream>>>(p);

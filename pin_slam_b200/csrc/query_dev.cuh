@@ -2,11 +2,8 @@
 // the thread-per-query neighbour search over the probe index, feature-row movement, phase A1 of a 32-query tile.
 #pragma once
 #include <algorithm>
-#include <mutex>
 #include <string>
-#include <vector>
 
-#include "mlp.cuh"
 #include "mlp_chain.cuh"
 
 namespace pinb {
@@ -16,15 +13,15 @@ constexpr int WPB = 12;  // warps per CTA (one CTA per SM): 12 x 32 threads x 16
 constexpr int REMAP = PINB200_REC_REMAP;
 
 struct QueryLayout {  // float offsets into dynamic smem
-  ChainDecSmem dec;
+  WarpDecSmem dec;
   int delta, warp0, n_warps, total;  // CTA-shared part, then n_warps per-warp blocks (WarpLay<FT>)
 };
 
 // Per-warp tile state, compile-time offsets (floats) so that every access is base + immediate.
 template <int FT>
 struct WarpLay {
-  static constexpr int KP0 = (FT + 3 + 7) / 8 * 8;
-  static constexpr int LDX = KP0 <= 8 ? 8 : ((KP0 - 8 + 31) / 32) * 32 + 8;
+  static constexpr int KP0 = dec_in_pad(FT);
+  static constexpr int LDX = ld8mod32(KP0);
   static constexpr int x = 0;                      // [32][LDX] decoder input rows / input gradient
   static constexpr int stash = x + WT * LDX;       // Stash block (see a1_tile)
   static constexpr int a = stash + 1536;           // [K][32] <g_xbar, f_k>

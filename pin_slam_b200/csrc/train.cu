@@ -14,8 +14,6 @@
 // Replaces the autograd reverse pass of utils/mapper.py:816-817 through
 // model/neural_points.py:597-731 (index_put_ accumulate) and model/decoder.py:61-85.
 #include <algorithm>
-#include <mutex>
-#include <vector>
 
 #include "mlp.cuh"
 
@@ -39,9 +37,14 @@ struct TrainParams {
   const float* knn_w;
   const float* dl;  // [N, out_dim] d loss / d decoder output (after out_scale / sigmoid)
   long long n;
-  // n_acc: length of the per-CTA shared-memory gradient accumulator, laid out [w0 | b0 | w1 | b1 | ... | w_out | b_out]
-  // with a slot for every bias whether the decoder has it or not (the bias sums are computed either way)
-  int K, wf, n_tiles, qpt, n_acc;
+  int K, wf, n_tiles, qpt;
+  // the per-CTA shared-memory gradient accumulator: n_acc floats laid out [w0 | b0 | w1 | b1 | ... | w_out | b_out],
+  // with a slot for every bias whether the decoder has it or not (the bias sums are computed either way); acc_*:
+  // offset of each block
+  int n_acc;
+  int acc_w[PINB200_MAX_HIDDEN_LAYERS];
+  int acc_b[PINB200_MAX_HIDDEN_LAYERS];
+  int acc_wout, acc_bout;
   float* grad_feat;
   // where each parameter block's gradient goes in the caller's flat gradient vector, whose layout has no slot for an
   // absent bias (pinb200_decoder_param_count); NULL: the bias is absent and its partial sums are dropped
@@ -121,17 +124,15 @@ __global__ void __launch_bounds__(TILE, PINB_K2_MIN_CTAS) train_bwd_kernel(const
   for (int e = tid; e < p.n_acc; e += TILE) s_dW[e] = 0.f;
   __syncthreads();
 
-  // offsets of each parameter block in the accumulator
+  // accumulator block offsets (TrainParams::acc_*), copied once: read from the kernel parameters at their uses in
+  // the layer loops they cost this kernel more spills (ptxas -v)
   int off_w[PINB200_MAX_HIDDEN_LAYERS], off_b[PINB200_MAX_HIDDEN_LAYERS];
-  int off = 0;
 #pragma unroll
   for (int l = 0; l < PINB200_MAX_HIDDEN_LAYERS; ++l) {
-    const int in = l == 0 ? D : H;
-    off_w[l] = off;
-    off_b[l] = off + H * in;
-    if (l < L) off += H * in + H;
+    off_w[l] = p.acc_w[l];
+    off_b[l] = p.acc_b[l];
   }
-  const int off_wout = off, off_bout = off + OC * H;
+  const int off_wout = p.acc_wout, off_bout = p.acc_bout;
 
   const int QPT = p.qpt;
   // feature rows are 16-byte aligned multiples of 4 floats: vector loads and vector reductions
@@ -413,32 +414,34 @@ static int launch_train(TrainParams& p, cudaStream_t stream) {
     return PINB200_ERR_UNSUPPORTED;
   }
   auto kern = train_bwd_kernel<H, DP>;
-  struct Cached {
-    int dev, occ;
-    size_t smem;
-  };
-  static std::mutex mu;
-  static std::vector<Cached> cache;
-  int occ = 0, dev = 0;
-  cudaGetDevice(&dev);
-  {
-    std::lock_guard<std::mutex> lk(mu);
-    for (const Cached& c : cache)
-      if (c.dev == dev && c.smem == smem_bytes) occ = c.occ;
-    if (occ == 0) {
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-      if (e != cudaSuccess) {
-        set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-        return PINB200_ERR_CUDA;
-      }
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, TILE, smem_bytes);
-      if (occ < 1) occ = 1;
-      cache.push_back({dev, occ, smem_bytes});
-    }
-  }
+  int occ = 1;
+  if (const int rc = prepare_kernel((const void*)kern, "train_bwd_kernel", smem_bytes, TILE, &occ)) return rc;
   const int grid = (int)std::min<long long>(p.n_tiles, (long long)sm_count() * occ);
   kern<<<grid, TILE, smem_bytes, stream>>>(p);
   return check_launch("train_bwd_kernel");
+}
+
+// the tensor-core kernel for 1-2 hidden layers over a 16-byte aligned feature table, the SIMT kernel (by padded
+// decoder input width) otherwise
+static int dispatch_train(TrainParams& p, cudaStream_t st) {
+  const int F = p.map.feature_dim, L = p.dec.n_hidden, D = p.dec.in_dim;
+  const bool aligned = (reinterpret_cast<uintptr_t>(p.feat) & 15) == 0;
+  if (aligned && (L == 1 || L == 2)) {
+    switch (F) {
+      case 4: return L == 1 ? launch_train_mma<4, 1>(p, st) : launch_train_mma<4, 2>(p, st);
+      case 8: return L == 1 ? launch_train_mma<8, 1>(p, st) : launch_train_mma<8, 2>(p, st);
+      case 16: return L == 1 ? launch_train_mma<16, 1>(p, st) : launch_train_mma<16, 2>(p, st);
+      case 32: return L == 1 ? launch_train_mma<32, 1>(p, st) : launch_train_mma<32, 2>(p, st);
+      case 64: return L == 1 ? launch_train_mma<64, 1>(p, st) : launch_train_mma<64, 2>(p, st);
+      default: break;
+    }
+  }
+  if (D <= 12) return launch_train<64, 12>(p, st);
+  if (D <= 20) return launch_train<64, 20>(p, st);
+  if (D <= 36) return launch_train<64, 36>(p, st);
+  if (D <= 68) return launch_train<64, 68>(p, st);
+  set_error("decoder in_dim %d unsupported (<= 68)", D);
+  return PINB200_ERR_UNSUPPORTED;
 }
 
 }  // namespace pinb
@@ -483,33 +486,28 @@ extern "C" int pinb200_train_backward(const pinb200_map_view* map, const pinb200
   p.n_tiles = (int)((n + p.qpt - 1) / p.qpt);
   p.grad_feat = grad_feat;
   {
+    // each parameter block's place in the shared-memory accumulator (acc) and in the caller's gradient vector (g)
     const int H = dec->hidden_dim;
     int acc = 0;
     float* g = grad_dec;
     for (int l = 0; l < dec->n_hidden; ++l) {
       const int nw = H * (l == 0 ? dec->in_dim : H);
+      p.acc_w[l] = acc;
       p.gd_w[l] = g;
+      acc += nw;
       g += nw;
+      p.acc_b[l] = acc;
       p.gd_b[l] = dec->b[l] ? g : nullptr;
+      acc += H;
       if (dec->b[l]) g += H;
-      acc += nw + H;
     }
+    p.acc_wout = acc;
     p.gd_wout = g;
+    acc += dec->out_dim * H;
     g += dec->out_dim * H;
+    p.acc_bout = acc;
     p.gd_bout = dec->b_out ? g : nullptr;
-    p.n_acc = acc + dec->out_dim * H + dec->out_dim;
+    p.n_acc = acc + dec->out_dim;
   }
-  const int D = dec->in_dim;
-  cudaStream_t st = (cudaStream_t)stream;
-  {
-    bool handled = false;  // tensor-core kernel for the common decoder shapes, SIMT kernel otherwise
-    const int rc = dispatch_train_mma(p, st, &handled);
-    if (handled) return rc;
-  }
-  if (D <= 12) return launch_train<64, 12>(p, st);
-  if (D <= 20) return launch_train<64, 20>(p, st);
-  if (D <= 36) return launch_train<64, 36>(p, st);
-  if (D <= 68) return launch_train<64, 68>(p, st);
-  set_error("decoder in_dim %d unsupported (<= 68)", D);
-  return PINB200_ERR_UNSUPPORTED;
+  return dispatch_train(p, (cudaStream_t)stream);
 }

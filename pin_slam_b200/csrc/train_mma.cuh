@@ -1,5 +1,5 @@
 // K2 on the tensor cores: the training backward pass with every contraction issued as warp-level
-// mma.sync.m16n8k8 TF32 instructions (3xTF32 split, fp32 accumulate -- see mlp_mma.cuh).
+// mma.sync.m16n8k8 TF32 instructions (3xTF32 split, fp32 accumulate -- see mlp_chain.cuh).
 //
 // A CTA is 4 warps and works on 128-row tiles (row = query when weighted_first, else (query, neighbour) pair):
 //   A   thread per row : re-gather the decoder input row from the saved kNN (float4 feature-row loads)
@@ -17,14 +17,14 @@
 // Replaces the autograd reverse pass of utils/mapper.py:816-817 through model/neural_points.py:597-731
 // (index_put_ accumulate) and model/decoder.py:61-85.  Included by train.cu (needs TrainParams).
 #pragma once
-#include "mlp_mma.cuh"
+#include "mlp_chain.cuh"
 
 namespace pinb {
 
 constexpr int LDH = 68;  // leading dimension of the hidden-activation tiles (== 4 mod 32)
 
 struct TrainMmaLayout {
-  MmaDecSmem dec;
+  WarpDecSmem dec;
   int x, h, dW, go, idx, w, total;
 };
 
@@ -95,7 +95,7 @@ __global__ void __launch_bounds__(TILE, train_mma_min_ctas<FT, LT>()) train_bwd_
                                                                 const TrainMmaLayout lay) {
   constexpr int H = 64;
   constexpr int F = FT, D = FT + 3;
-  constexpr int KP0 = (D + 7) / 8 * 8, KT0 = KP0 / 8, LDX = KP0 + 4;
+  constexpr int KP0 = dec_in_pad(FT), KT0 = KP0 / 8, LDX = KP0 + 4;
   extern __shared__ __align__(16) float smem[];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const pinb200_map_view& m = p.map;
@@ -110,13 +110,9 @@ __global__ void __launch_bounds__(TILE, train_mma_min_ctas<FT, LT>()) train_bwd_
   int* s_idx = reinterpret_cast<int*>(smem + lay.idx);
   float* s_w = smem + lay.w;
 
-  stage_mma_decoder(p.dec, lay.dec, smem);
+  stage_warp_decoder(p.dec, lay.dec, smem);
   for (int e = tid; e < p.n_acc; e += TILE) s_dW[e] = 0.f;
   __syncthreads();
-
-  // accumulator layout [w0 | b0 | (w1 | b1) | w_out | b_out] (TrainParams::n_acc)
-  const int off_b0 = H * D, off_b1 = off_b0 + H + H * H;
-  const int off_wout = LT == 1 ? off_b0 + H : off_b1 + H, off_bout = off_wout + OC * H;
 
   float dacc0[KT0][4];
   float dacc1[LT == 2 ? 8 : 1][4];
@@ -229,13 +225,13 @@ __global__ void __launch_bounds__(TILE, train_mma_min_ctas<FT, LT>()) train_bwd_
     float acc[2][8][4];
     uint64_t mk[LT];
     warp_gemm_3xtf32<KT0, 8, false, LDX>(acc, xw, smem + lay.dec.whi[0], smem + lay.dec.wlo[0], lay.dec.ldw[0], lane);
-    mk[0] = bias_act_frags<8>(acc, smem + lay.dec.b[0], leaky, lane);
+    mk[0] = bias_act_chain<8>(acc, smem + lay.dec.b[0], leaky, lane);
     if constexpr (LT == 2) {
       float* h0w = s_h + warp * 32 * LDH;
       store_frags<8, LDH>(h0w, acc, lane);  // h_0: input of layer 1 and of dW_1
       __syncwarp();
       warp_gemm_3xtf32<8, 8, false, LDH>(acc, h0w, smem + lay.dec.whi[1], smem + lay.dec.wlo[1], lay.dec.ldw[1], lane);
-      mk[LT - 1] = bias_act_frags<8>(acc, smem + lay.dec.b[1], leaky, lane);
+      mk[LT - 1] = bias_act_chain<8>(acc, smem + lay.dec.b[1], leaky, lane);
     }
     // d loss / d pre-output per row (sigmoid heads need the output value), output-layer gradients
     {
@@ -297,7 +293,7 @@ __global__ void __launch_bounds__(TILE, train_mma_min_ctas<FT, LT>()) train_bwd_
             v += __shfl_xor_sync(FULL, v, 4);
             v += __shfl_xor_sync(FULL, v, 8);
             v += __shfl_xor_sync(FULL, v, 16);
-            if (lane < 4) atomicAdd(s_dW + off_wout + c * H + nt * 8 + 2 * lane + e, v);
+            if (lane < 4) atomicAdd(s_dW + p.acc_wout + c * H + nt * 8 + 2 * lane + e, v);
           }
         float b = 0.f;
 #pragma unroll
@@ -309,7 +305,7 @@ __global__ void __launch_bounds__(TILE, train_mma_min_ctas<FT, LT>()) train_bwd_
               if (cc == c) b += gor[mt][hh][cc];
         if ((lane & 3) != 0) b = 0.f;  // the 4 lanes of a quad hold the same rows
         b = warp_sum(b);
-        if (lane == 0) atomicAdd(s_dW + off_bout + c, b);
+        if (lane == 0) atomicAdd(s_dW + p.acc_bout + c, b);
       }
       // G_{L-1} = mask * (go w_out)
 #pragma unroll
@@ -324,22 +320,22 @@ __global__ void __launch_bounds__(TILE, train_mma_min_ctas<FT, LT>()) train_bwd_
               if (c < OC) v = fmaf(gor[mt][e >> 1][c], wo[c * H + frag_col(nt, e, lane)], v);
             acc[mt][nt][e] = v;
           }
-      mask_frags<8>(acc, mk[LT - 1], leaky);
+      mask_chain<8>(acc, mk[LT - 1], leaky);
     }
 
     // ---------------- C: hidden layers, last to first ----------------
     if constexpr (LT == 2) {
       float* g1 = s_h + TILE * LDH;  // G_1 tile
-      frag_colsum_to_smem(acc, s_dW + off_b1, lane);
+      frag_colsum_to_smem(acc, s_dW + p.acc_b[1], lane);
       store_frags<8, LDH>(g1 + warp * 32 * LDH, acc, lane);
       __syncthreads();  // G_1 and h_0 of all 128 rows are in place
       dw_gemm_3xtf32<8, LDH, LDH>(dacc1, g1, warp * 16, s_h, lane);
       warp_gemm_3xtf32<8, 8, true, LDH>(acc, g1 + warp * 32 * LDH, smem + lay.dec.whi[1], smem + lay.dec.wlo[1],
                                         lay.dec.ldw[1], lane);
-      mask_frags<8>(acc, mk[0], leaky);
+      mask_chain<8>(acc, mk[0], leaky);
       __syncthreads();  // everyone is done reading h_0
     }
-    frag_colsum_to_smem(acc, s_dW + off_b0, lane);
+    frag_colsum_to_smem(acc, s_dW + p.acc_b[0], lane);
     store_frags<8, LDH>(s_h + warp * 32 * LDH, acc, lane);  // G_0 over h_0
     __syncthreads();  // G_0 and x of all 128 rows are in place
     dw_gemm_3xtf32<KT0, LDH, LDX>(dacc0, s_h, warp * 16, s_x, lane);
@@ -387,24 +383,25 @@ __global__ void __launch_bounds__(TILE, train_mma_min_ctas<FT, LT>()) train_bwd_
   flush_slab<KT0>(dacc0, p.gd_w[0], warp * 16, D, lane);
   if constexpr (LT == 2) flush_slab<8>(dacc1, p.gd_w[1], warp * 16, H, lane);
   __syncthreads();
-  flush_block(s_dW + off_b0, H, p.gd_b[0], tid);
-  if constexpr (LT == 2) flush_block(s_dW + off_b1, H, p.gd_b[1], tid);
-  flush_block(s_dW + off_wout, OC * H, p.gd_wout, tid);
-  flush_block(s_dW + off_bout, OC, p.gd_bout, tid);
+  flush_block(s_dW + p.acc_b[0], H, p.gd_b[0], tid);
+  if constexpr (LT == 2) flush_block(s_dW + p.acc_b[1], H, p.gd_b[1], tid);
+  flush_block(s_dW + p.acc_wout, OC * H, p.gd_wout, tid);
+  flush_block(s_dW + p.acc_bout, OC, p.gd_bout, tid);
 }
 
 template <int FT, int LT>
 static int launch_train_mma(TrainParams& p, cudaStream_t stream) {
-  constexpr int D = FT + 3, KP0 = (D + 7) / 8 * 8, LDX = KP0 + 4;
+  constexpr int LDX = dec_in_pad(FT) + 4;
   TrainMmaLayout l{};
-  l.dec = plan_mma_decoder_smem(p.dec, KP0, 0);
-  int o = align4i(l.dec.end);
+  // leading dimensions == 4 (mod 32): conflict-free scalar fragment loads in warp_gemm_3xtf32
+  l.dec = plan_warp_decoder_smem(p.dec, dec_in_pad(FT), 0, [](int k) { return k + 4; });
+  int o = align4(l.dec.end);
   l.x = o;
   o += TILE * LDX;
   l.h = o;
   o += LT * TILE * LDH;
   l.dW = o;
-  o += align4i(p.n_acc);
+  o += align4(p.n_acc);
   l.go = o;
   o += TILE * 4;
   l.idx = o;
@@ -418,60 +415,11 @@ static int launch_train_mma(TrainParams& p, cudaStream_t stream) {
     return PINB200_ERR_UNSUPPORTED;
   }
   auto kern = train_bwd_mma_kernel<FT, LT>;
-  struct Cached {
-    int dev, occ;
-    size_t smem;
-  };
-  static std::mutex mu;
-  static std::vector<Cached> cache;
-  int occ = 0, dev = 0;
-  cudaGetDevice(&dev);
-  {
-    std::lock_guard<std::mutex> lk(mu);
-    for (const Cached& c : cache)
-      if (c.dev == dev && c.smem == smem_bytes) occ = c.occ;
-    if (occ == 0) {
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-      if (e != cudaSuccess) {
-        set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-        return PINB200_ERR_CUDA;
-      }
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, TILE, smem_bytes);
-      if (occ < 1) occ = 1;
-      cache.push_back({dev, occ, smem_bytes});
-    }
-  }
+  int occ = 1;
+  if (const int rc = prepare_kernel((const void*)kern, "train_bwd_mma_kernel", smem_bytes, TILE, &occ)) return rc;
   const int grid = (int)std::min<long long>(p.n_tiles, (long long)sm_count() * occ);
   kern<<<grid, TILE, smem_bytes, stream>>>(p, l);
   return check_launch("train_bwd_mma_kernel");
-}
-
-// feature width / depth combinations with a tensor-core instantiation; everything else takes the SIMT kernel
-static int dispatch_train_mma(TrainParams& p, cudaStream_t st, bool* handled) {
-  *handled = true;
-  const int F = p.map.feature_dim, L = p.dec.n_hidden;
-  const bool aligned = (reinterpret_cast<uintptr_t>(p.feat) & 15) == 0;
-  if (aligned && L == 1) {
-    switch (F) {
-      case 4: return launch_train_mma<4, 1>(p, st);
-      case 8: return launch_train_mma<8, 1>(p, st);
-      case 16: return launch_train_mma<16, 1>(p, st);
-      case 32: return launch_train_mma<32, 1>(p, st);
-      case 64: return launch_train_mma<64, 1>(p, st);
-      default: break;
-    }
-  } else if (aligned && L == 2) {
-    switch (F) {
-      case 4: return launch_train_mma<4, 2>(p, st);
-      case 8: return launch_train_mma<8, 2>(p, st);
-      case 16: return launch_train_mma<16, 2>(p, st);
-      case 32: return launch_train_mma<32, 2>(p, st);
-      case 64: return launch_train_mma<64, 2>(p, st);
-      default: break;
-    }
-  }
-  *handled = false;
-  return PINB200_OK;
 }
 
 }  // namespace pinb

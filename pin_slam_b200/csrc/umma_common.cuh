@@ -6,7 +6,7 @@
 // c = l % 4 holds for every 8-column block j: d[4j + 0, 1] = rows 16w + g, columns 8j + 2c, 8j + 2c + 1 and
 // d[4j + 2, 3] = row 16w + g + 8, same columns.
 #pragma once
-#include "mlp_mma.cuh"
+#include "mlp_chain.cuh"  // TF32_MASK, dec_in_pad
 
 namespace pinb {
 
@@ -115,7 +115,7 @@ __device__ __forceinline__ void um_stage_weight(const float* __restrict__ src, i
 
 template <int FT>
 struct UmmaDims {
-  static constexpr int K0 = (FT + 3 + 7) / 8 * 8;  // decoder input width padded to the MMA k-step
+  static constexpr int K0 = dec_in_pad(FT);
 };
 
 }  // namespace pinb

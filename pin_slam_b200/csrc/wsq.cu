@@ -638,21 +638,7 @@ static int launch_wsq(QueryParams& p, cudaStream_t stream) {
     return PINB200_ERR_UNSUPPORTED;
   }
   auto kern = wsq_decode_kernel<FT, GRAD, PROF>;
-  static std::mutex mu;
-  static std::vector<int> done;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  {
-    std::lock_guard<std::mutex> lk(mu);
-    if (std::find(done.begin(), done.end(), dev) == done.end()) {
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-      if (e != cudaSuccess) {
-        set_error("cudaFuncSetAttribute(wsq_decode): %s", cudaGetErrorString(e));
-        return PINB200_ERR_CUDA;
-      }
-      done.push_back(dev);
-    }
-  }
+  if (const int rc = prepare_kernel((const void*)kern, "wsq_decode_kernel", smem_bytes)) return rc;
   p.qpt = WT;
   p.n_tiles = (int)((p.n + WT - 1) / WT);
   constexpr int QT = GRAD ? 32 : 128;

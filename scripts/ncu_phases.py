@@ -20,7 +20,7 @@ marks = [("prologue", 1), ("A1 probe loop", line_of("knn_search_lane(const")), (
          ("C2 chain rule + outputs", line_of("C1: a_k = <g_xbar")), ("other kernels", line_of("search-only kernels"))]
 def phase_of(f, ln):
     if f == "knn_select.cuh": return "A1 sorting networks"
-    if f in ("mlp_chain.cuh", "mlp_mma.cuh"): return "B decoder MMA (mlp_chain.cuh)"
+    if f == "mlp_chain.cuh": return "B decoder MMA (mlp_chain.cuh)"
     if f == "common.cuh": return "A1 hash / misc (common.cuh)"
     if f != "query.cu": return "intrinsics / other headers"
     name = marks[0][0]

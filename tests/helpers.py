@@ -210,8 +210,8 @@ def queries_near(m, n, seed, sigma=0.15):
 # ---------------------------------------------------------------------------
 def train_bwd_kernel_name(F, L, aligned=True):
     """The K2 kernel pinb200_train_backward launches for a 64-wide decoder with L hidden layers on F features
-    (dispatch_train_mma in train_mma.cuh: 1-2 layers on a 16-byte aligned feature table; else the SIMT kernel by padded
-    input width in train.cu)."""
+    (dispatch_train in train.cu: the tensor-core kernel for 1-2 layers on a 16-byte aligned feature table, else the
+    SIMT kernel by padded input width)."""
     if L <= 2 and aligned:
         return f"train_bwd_mma_kernel<{F}, {L}>"
     return f"train_bwd_kernel<64, {next(dp for dp in (12, 20, 36, 68) if F + 3 <= dp)}>"

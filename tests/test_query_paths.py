@@ -103,7 +103,7 @@ def case_id(c):
 
 def source_instantiations():
     """Kernel instantiations the dispatch code launches (the wsq_decode_kernel profiling variants excluded)."""
-    src = {f: open(os.path.join(CSRC, f)).read() for f in ("query.cu", "wsq.cu", "train.cu", "train_mma.cuh")}
+    src = {f: open(os.path.join(CSRC, f)).read() for f in ("query.cu", "wsq.cu", "train.cu")}
     q = src["query.cu"]
     names = {f"query_kernel<{F}, {wf}, {sp}>" for F in re.findall(r"launch_query<(\d+), WF, SPLIT>\(", q)
              for wf, sp in re.findall(r"dispatch_query_wf<(true|false), (true|false)>\(", q)}
@@ -111,8 +111,7 @@ def source_instantiations():
     names |= {f"wsq_decode_kernel<{F}, {g}, false>"
               for F, g, prof in re.findall(r"launch_wsq<(\d+), (true|false), (true|false)>\(", src["wsq.cu"])
               if prof == "false"}
-    names |= {f"train_bwd_mma_kernel<{F}, {L}>" for F, L in re.findall(r"launch_train_mma<(\d+), (\d+)>\(",
-                                                                          src["train_mma.cuh"])}
+    names |= {f"train_bwd_mma_kernel<{F}, {L}>" for F, L in re.findall(r"launch_train_mma<(\d+), (\d+)>\(", src["train.cu"])}
     names |= {f"train_bwd_kernel<{H}, {DP}>" for H, DP in re.findall(r"launch_train<(\d+), (\d+)>\(", src["train.cu"])}
     return names
 

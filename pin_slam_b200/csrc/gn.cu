@@ -312,7 +312,8 @@ extern "C" int pinb200_gn_step(const float* xyz, const float* sdf, const float* 
                                const float* color_pred, const float* color_grad, int32_t color_channels,
                                int32_t color_mode, float w_photo, double* sums, double* result, double* t_inout,
                                void* stream) {
-  if (!xyz || !sdf || !grad || !nn_count || !sums || !result || n < 0) {
+  // n == 0 (empty tensors have null data pointers) takes gn_solve_kernel: identity step, T unchanged
+  if ((n > 0 && (!xyz || !sdf || !grad || !nn_count)) || !sums || !result || n < 0) {
     set_error("gn_step: null argument");
     return PINB200_ERR_BAD_ARG;
   }

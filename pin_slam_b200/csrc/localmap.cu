@@ -57,10 +57,10 @@ __global__ void __launch_bounds__(LM_TPB) local_keep_kernel(const LocalSel p) {
   if (i < p.n) {
     const bool recent = p.mask[i] || (p.temporal_on && p.counts[0] < 100);  // fewer than 100 recent points: keep all
     bool near;
-    if (p.sensor_f64) {  // float32 points minus a float64 sensor position: torch promotes to float64
+    if (p.sensor_f64) {  // float32 points minus a float64 sensor position: torch promotes to float64 (no DFMA)
       const double* s = reinterpret_cast<const double*>(p.sensor);
       const double dx = (double)p.points[3 * i] - s[0], dy = (double)p.points[3 * i + 1] - s[1], dz = (double)p.points[3 * i + 2] - s[2];
-      near = (dx * dx + dy * dy) + dz * dz < p.radius2_d;
+      near = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)) < p.radius2_d;
     } else {
       const float* s = reinterpret_cast<const float*>(p.sensor);
       const float dx = __fsub_rn(p.points[3 * i], s[0]), dy = __fsub_rn(p.points[3 * i + 1], s[1]), dz = __fsub_rn(p.points[3 * i + 2], s[2]);
@@ -138,8 +138,9 @@ extern "C" int pinb200_local_map_select(const float* points, const int32_t* ts_c
                                         int32_t use_mid_ts, int32_t use_travel_dist, int32_t diff_ts_local, int32_t reboot_map,
                                         int32_t reboot_ts, float diff_travel, const void* sensor_pos, int32_t sensor_is_f64,
                                         double radius2, uint8_t* local_mask, int32_t* scratch, int64_t* counts, void* stream) {
-  if (!points || !sensor_pos || !local_mask || !scratch || !counts || n < 0 ||
-      (temporal_on && (!ts_create || (use_mid_ts && !ts_update) || (use_travel_dist && !travel_dist)))) {
+  // an empty map (torch gives its tensors a null data pointer) still writes the padding row's mask and the counts
+  if ((n > 0 && !points) || !sensor_pos || !local_mask || !scratch || !counts || n < 0 ||
+      (temporal_on && n > 0 && (!ts_create || (use_mid_ts && !ts_update) || (use_travel_dist && !travel_dist)))) {
     set_error("local_map_select: bad argument");
     return PINB200_ERR_BAD_ARG;
   }
@@ -178,7 +179,8 @@ extern "C" int pinb200_local_map_gather(const float* points, const float* orient
                                         int64_t n_local, int32_t miss_value, int64_t* idx_pad, int32_t* global2local,
                                         float* l_points, float* l_orient, float* l_certainty, int32_t* l_ts_update,
                                         void* stream) {
-  if (!points || !orient || !certainty || !ts_update || !local_mask || !scratch || !idx_pad || !global2local || n < 0 ||
+  if ((n > 0 && (!points || !orient || !certainty || !ts_update)) || !local_mask || !scratch || !idx_pad ||
+      !global2local || n < 0 ||
       n_local < 0 || (n_local > 0 && (!l_points || !l_orient || !l_certainty || !l_ts_update))) {
     set_error("local_map_gather: bad argument");
     return PINB200_ERR_BAD_ARG;

@@ -4,7 +4,8 @@
 // time.  Here the pool lives in two fixed-capacity arenas (pin_slam_b200/utils/mapper.py: _PoolArena) and the filter
 // is ONE order-preserving compaction from one arena into the other: flags + block sums, a scan of the block sums,
 // and a scatter of all arrays.  The distance test uses the reference's arithmetic (the pool is fp32, the sensor
-// origin fp64: torch promotes the difference to fp64).
+// origin fp64: torch promotes the difference to fp64), every product and sum rounded on its own: a contracted DFMA
+// would decide samples within an ulp of the radius differently from torch.
 #include <algorithm>
 
 #include "scan.cuh"
@@ -26,7 +27,7 @@ struct PoolPtrs {
 __device__ __forceinline__ bool pool_keep(const float* __restrict__ g, long long i, const double* __restrict__ origin,
                                           double r2) {
   const double dx = (double)g[3 * i] - origin[0], dy = (double)g[3 * i + 1] - origin[1], dz = (double)g[3 * i + 2] - origin[2];
-  return (dx * dx + dy * dy) + dz * dz < r2;
+  return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)) < r2;
 }
 
 __global__ void __launch_bounds__(PF_TPB) pool_count_kernel(const float* __restrict__ gcoord, long long n,

@@ -308,7 +308,8 @@ def test_cuda_radius_search_with_time_filter_matches_reference():
     assert np.array_equal(idxg.cpu().numpy().astype(np.int32), fx["rs_nofilter.idx"])
 
 
-@pytest.mark.parametrize("n,voxel", [(65536, 0.08), (45000, 0.6), (3000, 0.4), (17, 0.4), (200000, 0.05)])
+@pytest.mark.parametrize("n,voxel", [(65536, 0.08), (45000, 0.6), (3000, 0.4), (17, 0.4), (200000, 0.05),
+                                     (1_200_000, 0.2), (300000, 64.0)])
 def test_cuda_voxel_downsample_equals_reference_formulation(n, voxel):
     """pinb200_voxel_downsample (hash set + compaction + sort of the winners) returns exactly what the reference's
     unique / scatter-amin formulation returns (utils/tools.py:583-668): same winners, same ascending-key order, for the
@@ -319,6 +320,8 @@ def test_cuda_voxel_downsample_equals_reference_formulation(n, voxel):
     g = torch.Generator().manual_seed(n)
     pts = (torch.rand(n, 3, generator=g) * torch.tensor([40.0, 30.0, 6.0]) - torch.tensor([20.0, 15.0, 1.0]))
     pts[n // 2:n // 2 + n // 10] = pts[:n // 10]  # exact duplicates: ties on the quantised distance
+    if voxel > 40.0:  # a voxel larger than the frame: shifted into one voxel, every thread contends for one slot
+        pts = pts - pts.min(0).values
     val = torch.randint(0, 50, (n,), generator=g).float()
     cpu_a = npmod.voxel_down_sample(pts, voxel)              # torch formulation (CPU tensors take that path)
     cpu_b = npmod.voxel_down_sample_min_value(pts, voxel, val)

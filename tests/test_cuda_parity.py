@@ -443,20 +443,23 @@ def test_train_backward_vs_autograd_synthetic(F, K, L, wf, oc, pgo, leaky, bias,
 
 
 def test_adam_matches_torch():
-    g = torch.Generator().manual_seed(0)
-    p = torch.randn(5000, generator=g)
-    ref = p.clone().requires_grad_(True)
-    opt = torch.optim.Adam([ref], lr=0.01, betas=(0.9, 0.99), eps=1e-15)
-    pc, m, v = p.cuda(), torch.zeros(5000, device="cuda"), torch.zeros(5000, device="cuda")
-    for step in range(1, 6):
-        grad = torch.randn(5000, generator=g) * 1e-3
-        grad[::7] = 0.0
-        ref.grad = grad.clone()
-        opt.step()
-        gc = grad.cuda()
-        ops().adam_step(pc, gc, m, v, 0.01, 0.9, 0.99, 1e-15, 0.0, step)
-        assert float(gc.abs().max()) == 0.0  # zero_grad folded in
-    np.testing.assert_allclose(pc.cpu().numpy(), ref.detach().numpy(), rtol=2e-6, atol=2e-7)
+    """A small tensor, and a 106 k x 32 feature table with weight decay: past the grid-stride threshold of adam_kernel
+    (8 x SMs x 256 elements), where every thread updates several elements."""
+    for n, wd in ((5000, 0.0), (106_003 * 32, 1e-3)):
+        g = torch.Generator().manual_seed(0)
+        p = torch.randn(n, generator=g)
+        ref = p.clone().requires_grad_(True)
+        opt = torch.optim.Adam([ref], lr=0.01, betas=(0.9, 0.99), eps=1e-15, weight_decay=wd)
+        pc, m, v = p.cuda(), torch.zeros(n, device="cuda"), torch.zeros(n, device="cuda")
+        for step in range(1, 6):
+            grad = torch.randn(n, generator=g) * 1e-3
+            grad[::7] = 0.0
+            ref.grad = grad.clone()
+            opt.step()
+            gc = grad.cuda()
+            ops().adam_step(pc, gc, m, v, 0.01, 0.9, 0.99, 1e-15, wd, step)
+            assert float(gc.abs().max()) == 0.0  # zero_grad folded in
+        np.testing.assert_allclose(pc.cpu().numpy(), ref.detach().numpy(), rtol=2e-6, atol=2e-7)
 
 
 def _flat_handle(dec, sigmoid_out=False):

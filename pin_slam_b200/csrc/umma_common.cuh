@@ -98,13 +98,14 @@ __device__ __forceinline__ int um_kperm(int c) { return (c & ~7) | ((c & 1) ? 4 
 
 // stage the canonical K-major B tile of `rows` x `cols`: element (r, c) = src[r][c] for r < rows_src, c < cols_src,
 // zero elsewhere; `src_ld` = leading dimension of the row-major source.  `kperm` stores column c at um_kperm(c), for an
-// A operand taken from accumulator registers.
+// A operand taken from accumulator registers.  `transpose` stages the transposed source: element (r, c) = src[c][r].
 __device__ __forceinline__ void um_stage_weight(const float* __restrict__ src, int src_ld, int rows_src, int cols_src, int rows,
-                                                int cols, unsigned char* hi, unsigned char* lo, bool kperm = false) {
+                                                int cols, unsigned char* hi, unsigned char* lo, bool kperm = false,
+                                                bool transpose = false) {
   for (int e = threadIdx.x; e < rows * cols; e += blockDim.x) {
     const int r = e / cols, c = e - r * cols;
     float w = 0.f;
-    if (r < rows_src && c < cols_src) w = __ldg(src + (size_t)r * src_ld + c);
+    if (r < rows_src && c < cols_src) w = __ldg(src + (transpose ? (size_t)c * src_ld + r : (size_t)r * src_ld + c));
     const float h = __uint_as_float(__float_as_uint(w) & TF32_MASK);
     const int cs = kperm ? um_kperm(c) : c;
     const int off = (r >> 3) * ((cols >> 2) * UM_W_LBO) + (cs >> 2) * UM_W_LBO + (r & 7) * 16 + (cs & 3) * 4;

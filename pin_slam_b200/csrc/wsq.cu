@@ -24,6 +24,16 @@
 // no input-gradient tile, which is what makes room for a ring of A tiles: the gathers of later tiles run under the MMA
 // chain of tile t.  Without d/dq (mesher, dense RGB-D queries) a tile is 128 value rows.
 //
+// With a single output channel (the SDF head) d/dq takes the ADJOINT schedule instead: for a 2-layer head,
+// d out / d q_j = s v' . u_j with u_j = W0 (dx/dq_j) (the layer-0 tangent), ONE adjoint vector per query
+// v' = D0 W1^T (w_out . D1) (D = the (leaky-)ReLU derivative masks of the value row; L = 1: v' = D0 w_out) and s the
+// output scale or sigmoid derivative, so the tangent rows stop at layer 0: 108 instead of 156 wgmma per 64 queries.
+// Gather team h fills 64-query groups that consumer warpgroup h alone decodes: four fp32 blocks V, T1, T2, T3 of 64
+// rows each, row r of every block = query r, so a thread holds the same accumulator elements of the value rows, of v'
+// and of every u_j (no mask shuffle).  Layer 0 takes its A fragments from these blocks through registers (split into
+// hi / lo there: fp32 blocks are half the size of hi / lo tiles, which is what leaves room for the staged W1^T).
+// A colour Jacobian (3 channels) would need three adjoint vectors and save no MMA work, so it stays in forward mode.
+//
 // Replaces model/neural_points.py:598-731 (gathers, IDW, weighted_first), model/decoder.py:61-85,112 and the autograd
 // call of utils/tools.py:247-260 for batches of >= PINB200_SPLIT_MIN_QUERIES_WF queries (inference mode).
 #include "query_dev.cuh"
@@ -45,6 +55,12 @@ constexpr int WS_A0 = 2;       // A-tile ring slots, one per gather team
 // rewritten for tile i + WS_QX only after the A tile of tile i + WS_A0 was released, i.e. after every consumer warp
 // stored tile i
 constexpr int WS_QX = 2 * WS_A0;
+// adjoint schedule (d/dq of a single-output head): a group of 64 queries is four 64-row fp32 blocks V, T1, T2, T3 of
+// WS_LDA floats per row; WS_LDA == 4 (mod 32) keeps the consumers' scalar A-fragment loads free of bank conflicts.
+// Columns >= WS_LDA (the last four of K0 = 40) are zero and never stored
+constexpr int WS_QG = 64;
+constexpr int WS_LDA = 36;
+constexpr int WS_GBLK = WS_QG * WS_LDA;  // floats per block of a group
 
 struct WsMeta {  // float offsets inside a meta block of 32 queries, [field][k][lane]
   static constexpr int li = 0;                   // [8][32] neighbour id | REMAP, -1 invalid
@@ -58,8 +74,9 @@ struct WsMeta {  // float offsets inside a meta block of 32 queries, [field][k][
 };
 
 struct WsLayout {  // byte offsets from the dynamic shared memory base
-  int w0_hi, w0_lo, w1_hi, w1_lo, b0, b1, wout, bout;
-  int a0, a0_half, a0_stride;  // ring of A tiles: slot s = [a0 + s*stride: hi | + half: lo]
+  int adj;                     // 1: adjoint schedule (d/dq with one output channel), A slots are fp32 groups
+  int w0_hi, w0_lo, w1_hi, w1_lo, w1t_hi, w1t_lo, b0, b1, wout, bout;
+  int a0, a0_half, a0_stride;  // ring of A tiles: slot s = [a0 + s*stride: hi | + half: lo] (adjoint: one fp32 group)
   int qidx;                    // [WS_QX][128] original query index of every tile row's query
   int meta, meta_stride, n_meta;
   int bars, total;
@@ -74,8 +91,8 @@ constexpr int WSB_A0_FULL = 0, WSB_A0_EMPTY = WSB_A0_FULL + WS_A0, WSB_META_FULL
 // pinb200_debug_read("ws_profile", ...).  The last slot of every warp holds its role code (WS_ROLE_*), so that a
 // reader of the counters (scripts/exp_decode.py) follows the kernel's role layout.
 constexpr int WS_PROF_SLOTS = 8;
-// C consumer warps, G gather warps that also fill the meta ring
-constexpr int WS_ROLE_C = 1, WS_ROLE_G = 4;
+// C consumer warps (CA: of the adjoint schedule), G gather warps that also fill the meta ring
+constexpr int WS_ROLE_C = 1, WS_ROLE_CA = 2, WS_ROLE_G = 4;
 constexpr int WS_PROF_CTAS = 132;  // one CTA per SM of an H100 SXM
 __device__ unsigned long long g_ws_prof[WS_PROF_CTAS * (WS_THREADS / 32) * WS_PROF_SLOTS];
 static int g_ws_profile = 0;
@@ -187,8 +204,9 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
   using DM = UmmaDims<FT>;
   constexpr int K0 = DM::K0, F = FT, D = FT + 3;
   using M = RowMap<FT>;
-  constexpr int QT = GRAD ? 32 : 128;   // queries per tile
-  constexpr int BPT = QT / WT;          // meta blocks per tile
+  const bool adj = GRAD && lay.adj;     // adjoint schedule: tiles are 64-query groups, one per consumer warpgroup
+  const int QT = adj ? WS_QG : (GRAD ? 32 : 128);  // queries per tile
+  const int BPT = QT / WT;              // meta blocks per tile
   constexpr int MB = GRAD ? 8 : 16;     // meta ring slots (blocks of 32 queries; a value-only tile has 4)
   constexpr int MSTRIDE = GRAD ? WsMeta::floats_g : WsMeta::floats_ng;
   constexpr int NPASS = WT / M::RPP;    // gather passes per meta block (F = 32: 8 passes of 4 queries)
@@ -209,7 +227,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
     };
     for (int s = 0; s < WS_A0; ++s) {
       init(WSB_A0_FULL + s, WS_GW);
-      init(WSB_A0_EMPTY + s, WS_CW);
+      init(WSB_A0_EMPTY + s, adj ? 4 : WS_CW);  // adjoint: one warpgroup consumes a group
     }
     for (int s = 0; s < WS_MB_MAX; ++s) {
       init(WSB_META_FULL + s, 1);
@@ -219,6 +237,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
   }
   um_stage_weight(p.dec.w[0], D, H, D, H, K0, sm + lay.w0_hi, sm + lay.w0_lo);
   if (L > 1) um_stage_weight(p.dec.w[1], H, H, H, H, H, sm + lay.w1_hi, sm + lay.w1_lo, true);
+  if (adj && L > 1) um_stage_weight(p.dec.w[1], H, H, H, H, H, sm + lay.w1t_hi, sm + lay.w1t_lo, true, true);
   __syncthreads();
   // the layer-0 bias rides on the MMA: input column D is 1 for value rows (0 for tangent rows), weight column D = b0
   static_assert(D < K0, "a spare (padding) input column carries the bias");
@@ -264,25 +283,51 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
     const uint64_t w0h_d = um_desc(um_smem_u32(sm + lay.w0_hi), UM_W_LBO, W_SBO0), w0l_d = um_desc(um_smem_u32(sm + lay.w0_lo), UM_W_LBO, W_SBO0);
     const uint64_t w1h_d = um_desc(um_smem_u32(sm + lay.w1_hi), UM_W_LBO, W_SBO1), w1l_d = um_desc(um_smem_u32(sm + lay.w1_lo), UM_W_LBO, W_SBO1);
 
-    // bias (value rows; `bias` may be null) + ReLU gate of the 32 accumulator values of a half.  The gate of a tangent
-    // row is the sign pattern of its query's value row: the 32 sign bits travel in ONE shuffle.
-    auto gate = [&](float (&z)[32], const float* bias) {
+    // bias (times bs: 1 for value rows, 0 for tangent rows; `bias` may be null) + ReLU gate of the 32 accumulator
+    // values of a half; returns the sign pattern.  In a forward-mode tile (`interleaved`) the gate of a tangent row is
+    // the sign pattern of its query's value row: the 32 sign bits travel in ONE shuffle.
+    auto gate = [&](float (&z)[32], const float* bias, float bs, bool interleaved) {
       if (bias) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const float2 b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * c);
-          z[4 * j] = fmaf(bsel, b.x, z[4 * j]);
-          z[4 * j + 1] = fmaf(bsel, b.y, z[4 * j + 1]);
-          z[4 * j + 2] = fmaf(bsel, b.x, z[4 * j + 2]);
-          z[4 * j + 3] = fmaf(bsel, b.y, z[4 * j + 3]);
+          z[4 * j] = fmaf(bs, b.x, z[4 * j]);
+          z[4 * j + 1] = fmaf(bs, b.y, z[4 * j + 1]);
+          z[4 * j + 2] = fmaf(bs, b.x, z[4 * j + 2]);
+          z[4 * j + 3] = fmaf(bs, b.y, z[4 * j + 3]);
         }
       }
       uint32_t mk = 0u;
 #pragma unroll
       for (int e = 0; e < 32; ++e) mk |= z[e] > 0.f ? (1u << e) : 0u;
-      if (GRAD) mk = __shfl_sync(FULL, mk, src);
+      if (GRAD && interleaved) mk = __shfl_sync(FULL, mk, src);
 #pragma unroll
       for (int e = 0; e < 32; ++e) z[e] = ((mk >> e) & 1u) ? z[e] : slope * z[e];
+      return mk;
+    };
+    // D = A W^T (64 x 64 x 64, 3xTF32) with A the accumulator fragment `a` of a 64 x 64 activation (overwritten with
+    // its hi part) and W a weight staged with kperm: the accumulator fragment is the A fragment once the k order inside
+    // a k-step is permuted
+    auto mma_rs64 = [&](float (&a)[32], float (&d)[32], uint64_t wh_d, uint64_t wl_d) {
+      uint32_t lo[32];
+#pragma unroll
+      for (int e = 0; e < 32; ++e) {
+        d[e] = 0.f;
+        const float hi = __uint_as_float(__float_as_uint(a[e]) & TF32_MASK);
+        lo[e] = __float_as_uint(a[e] - hi);
+        a[e] = hi;
+      }
+      wg_fence();
+      ws_unroll<H / 8>([&](auto S) {
+        constexpr int s = decltype(S)::value, WO = s * W_STEP;
+        const uint32_t h0 = __float_as_uint(a[4 * s]), h1 = __float_as_uint(a[4 * s + 2]), h2 = __float_as_uint(a[4 * s + 1]),
+                       h3 = __float_as_uint(a[4 * s + 3]);
+        wg_mma_n64_rs_at<WO>(d, lo[4 * s], lo[4 * s + 2], lo[4 * s + 1], lo[4 * s + 3], wh_d, s > 0);  // small terms first
+        wg_mma_n64_rs_at<WO>(d, h0, h1, h2, h3, wl_d, 1);
+        wg_mma_n64_rs_at<WO>(d, h0, h1, h2, h3, wh_d, 1);
+      });
+      wg_commit();
+      wg_wait0();
     };
     // output head of the two rows of this thread (quad-reduced: every lane of the quad holds the sums)
     auto head = [&](const float (&z)[32], float (&o)[2][4]) {
@@ -354,69 +399,180 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       }
     };
 
-    int i = 0;
-    for (long long T = blockIdx.x; T < n_tiles; T += gridDim.x, ++i) {
-      const int slot = i % WS_A0;
-      ws_wait(um_smem_u32(bars + WSB_A0_FULL + slot), (uint32_t)(i / WS_A0) & 1u);
-      clk.lap(0);
-      // ---- layer 0 of this warpgroup's half, A tile from shared memory
-      float d0[32];
-#pragma unroll
-      for (int e = 0; e < 32; ++e) d0[e] = 0.f;
-      {
-        const uint32_t a_hi = um_smem_u32(sm + lay.a0 + slot * lay.a0_stride);
-        const uint64_t ah = um_desc(a_hi, UM_A_LBO, A_SBO0) + h * A_HALF, al = um_desc(a_hi + lay.a0_half, UM_A_LBO, A_SBO0) + h * A_HALF;
-        wg_fence();
+    if (adj) {
+      // ---------------------------------------------------------------------------------------------------
+      // Adjoint schedule (d/dq of a single-output head): warpgroup h consumes the groups i = h (mod 2) of this CTA,
+      // which gather team h fills into A slot h.  Row r of each block V, T1, T2, T3 of a group is query r, so the
+      // thread that holds element (r, col) of u_j = W0 T_j also holds it for the value rows and for
+      //   v' = D0 W1^T (w_out . D1)   (L = 1: D0 w_out),   and   d out / d q_j = v' . u_j:
+      // the tangents stop at layer 0 and need neither the value row's mask shuffle nor a second layer.
+      // profile slots: 0 wait A group, 1 value rows (layers, head, sdf), 2 adjoint, 3 tangents + gradient stores
+      // ---------------------------------------------------------------------------------------------------
+      const uint64_t w1th_d = um_desc(um_smem_u32(sm + lay.w1t_hi), UM_W_LBO, W_SBO1),
+                     w1tl_d = um_desc(um_smem_u32(sm + lay.w1t_lo), UM_W_LBO, W_SBO1);
+      const int row0 = 16 * wq + g8;  // this thread's rows of every block: row0, row0 + 8
+      float* out_v = p.is_color ? p.out.color : p.out.sdf;
+      float* out_g = p.is_color ? p.out.color_grad : p.out.grad;
+      float* out_s = p.is_color ? nullptr : p.out.sdf_std;
+      // layer 0 of one 64-row block: the A fragments come from the fp32 group and are split into hi / lo in registers
+      // (same 3xTF32 terms and order as an A tile stored hi / lo).  `release` frees the A slot once they are loaded
+      auto layer0 = [&](const float* blk, float (&d)[32], int slot, bool release) {
+        const float* r = blk + row0 * WS_LDA + c;
+        float a[K0 / 8][4];
         ws_unroll<K0 / 8>([&](auto S) {
-          constexpr int s = decltype(S)::value, AO = s * A_STEP, WO = s * W_STEP;
-          wg_mma_n64_at<AO, WO>(d0, al, w0h_d, s > 0);  // small terms first
-          wg_mma_n64_at<AO, WO>(d0, ah, w0l_d, 1);
-          wg_mma_n64_at<AO, WO>(d0, ah, w0h_d, 1);
+          constexpr int s = decltype(S)::value;
+          a[s][0] = r[8 * s];
+          a[s][1] = r[8 * WS_LDA + 8 * s];
+          if constexpr (8 * s + 4 < WS_LDA) {
+            a[s][2] = r[8 * s + 4];
+            a[s][3] = r[8 * WS_LDA + 8 * s + 4];
+          } else {
+            a[s][2] = a[s][3] = 0.f;
+          }
         });
-        wg_commit();
-        wg_wait0();
-      }
-      __syncwarp();
-      if (lane == 0) ws_arrive(um_smem_u32(bars + WSB_A0_EMPTY + slot));  // the gather team may refill the A tile
-      clk.lap(1);
-      float o[2][4];
-      if (L > 1) {
-        // ---- layer-0 epilogue (the bias came through the MMA): gated activations, hi / lo split in place -> layer 1
-        // with the A operand from registers
-        float d1[32];
-        uint32_t lo[32];
-#pragma unroll
-        for (int e = 0; e < 32; ++e) d1[e] = 0.f;
-        gate(d0, nullptr);
-#pragma unroll
-        for (int e = 0; e < 32; ++e) {
-          const float hi = __uint_as_float(__float_as_uint(d0[e]) & TF32_MASK);
-          lo[e] = __float_as_uint(d0[e] - hi);
-          d0[e] = hi;
+        if (release) {
+          __syncwarp();
+          if (lane == 0) ws_arrive(um_smem_u32(bars + WSB_A0_EMPTY + slot));  // the gather team may refill the slot
         }
-        wg_fence();
-        ws_unroll<H / 8>([&](auto S) {
+#pragma unroll
+        for (int e = 0; e < 32; ++e) d[e] = 0.f;
+        ws_unroll<K0 / 8>([&](auto S) {
           constexpr int s = decltype(S)::value, WO = s * W_STEP;
-          const uint32_t h0 = __float_as_uint(d0[4 * s]), h1 = __float_as_uint(d0[4 * s + 2]), h2 = __float_as_uint(d0[4 * s + 1]),
-                         h3 = __float_as_uint(d0[4 * s + 3]);
-          wg_mma_n64_rs_at<WO>(d1, lo[4 * s], lo[4 * s + 2], lo[4 * s + 1], lo[4 * s + 3], w1h_d, s > 0);
-          wg_mma_n64_rs_at<WO>(d1, h0, h1, h2, h3, w1l_d, 1);
-          wg_mma_n64_rs_at<WO>(d1, h0, h1, h2, h3, w1h_d, 1);
+          uint32_t hi[4], lo[4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            hi[k] = __float_as_uint(a[s][k]) & TF32_MASK;
+            lo[k] = __float_as_uint(a[s][k] - __uint_as_float(hi[k]));
+          }
+          wg_fence();
+          wg_mma_n64_rs_at<WO>(d, lo[0], lo[1], lo[2], lo[3], w0h_d, s > 0);  // small terms first
+          wg_mma_n64_rs_at<WO>(d, hi[0], hi[1], hi[2], hi[3], w0l_d, 1);
+          wg_mma_n64_rs_at<WO>(d, hi[0], hi[1], hi[2], hi[3], w0h_d, 1);
         });
         wg_commit();
         wg_wait0();
+      };
+
+      int i = h;
+      for (long long G = blockIdx.x + (long long)h * gridDim.x; G < n_tiles; G += (long long)WS_GT * gridDim.x, i += WS_GT) {
+        const int slot = i % WS_A0;
+        ws_wait(um_smem_u32(bars + WSB_A0_FULL + slot), (uint32_t)(i / WS_A0) & 1u);
+        clk.lap(0);
+        const float* grp = reinterpret_cast<const float*>(sm + lay.a0 + slot * lay.a0_stride);
+        // ---- value rows: layer 0 (bias through the MMA), gate, layer 1, head, sdf
+        float d0[32], v[32], o[2][4];
+        layer0(grp, d0, slot, false);
+        const uint32_t m0 = gate(d0, nullptr, 1.f, false);
+        if (L > 1) {
+          mma_rs64(d0, v, w1h_d, w1l_d);
+          const uint32_t m1 = gate(v, s_b1, 1.f, false);
+          head(v, o);
+          // g1 = w_out . D1, the A operand of the adjoint layer
+#pragma unroll
+          for (int e = 0; e < 32; ++e)
+            v[e] = s_wout[8 * (e >> 2) + 2 * c + (e & 1)] * (((m1 >> e) & 1u) ? 1.f : slope);
+        } else {
+          head(d0, o);
+#pragma unroll
+          for (int e = 0; e < 32; ++e) v[e] = s_wout[8 * (e >> 2) + 2 * c + (e & 1)];
+        }
+        // lane c = r of a quad stores the results of row r (r = 0, 1)
+        const bool st = c < 2 && G * QT + row0 + 8 * c < p.n;  // the tail of the last group carries no valid index
+        const long long qi = st ? s_qidx[(i % WS_QX) * QT + row0 + 8 * c] : 0;
+        float sc[2];  // d out / d (head sum) of the two rows
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const float oo = o[r][0] + s_bout[0];
+          float val;
+          if (p.dec.sigmoid_out) {
+            val = 1.f / (1.f + expf(-oo));
+            sc[r] = val * (1.f - val);
+          } else {
+            val = oo * p.dec.out_scale;
+            sc[r] = p.dec.out_scale;
+          }
+          if (st && c == r) {
+            if (out_v) out_v[qi] = val;
+            if (out_s) out_s[qi] = 0.f;
+          }
+        }
+        clk.lap(1);
+        // ---- adjoint: v' = D0 (W1^T g1), scaled by d out / d (head sum)
+        if (L > 1) {
+          mma_rs64(v, d0, w1th_d, w1tl_d);
+#pragma unroll
+          for (int e = 0; e < 32; ++e) v[e] = d0[e];
+        }
+#pragma unroll
+        for (int e = 0; e < 32; ++e) v[e] = (((m0 >> e) & 1u) ? v[e] : slope * v[e]) * sc[(e >> 1) & 1];
         clk.lap(2);
-        // ---- last hidden layer: bias, gate, output head(s), results
-        gate(d1, s_b1);
-        head(d1, o);
-        store(T, i, o);
-      } else {
-        // single hidden layer: its bias came through the MMA
-        gate(d0, nullptr);
-        head(d0, o);
-        store(T, i, o);
+        // ---- tangent rows: u_j = W0 T_j (T rows carry 0 in the bias column), d out / d q_j = v' . u_j
+        float* const gdst = st && out_g ? out_g + 3 * qi : nullptr;
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+          layer0(grp + (j + 1) * WS_GBLK, d0, slot, j == 2);
+          float g[2];
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            float acc = 0.f;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              acc = fmaf(v[4 * jj + 2 * r], d0[4 * jj + 2 * r], acc);
+              acc = fmaf(v[4 * jj + 2 * r + 1], d0[4 * jj + 2 * r + 1], acc);
+            }
+            acc += __shfl_xor_sync(FULL, acc, 1);
+            g[r] = acc + __shfl_xor_sync(FULL, acc, 2);
+          }
+          if (gdst) gdst[j] = c == 0 ? g[0] : g[1];
+        }
+        clk.lap(3);
       }
-      clk.lap(3);
+    } else {
+      int i = 0;
+      for (long long T = blockIdx.x; T < n_tiles; T += gridDim.x, ++i) {
+        const int slot = i % WS_A0;
+        ws_wait(um_smem_u32(bars + WSB_A0_FULL + slot), (uint32_t)(i / WS_A0) & 1u);
+        clk.lap(0);
+        // ---- layer 0 of this warpgroup's half, A tile from shared memory
+        float d0[32];
+#pragma unroll
+        for (int e = 0; e < 32; ++e) d0[e] = 0.f;
+        {
+          const uint32_t a_hi = um_smem_u32(sm + lay.a0 + slot * lay.a0_stride);
+          const uint64_t ah = um_desc(a_hi, UM_A_LBO, A_SBO0) + h * A_HALF, al = um_desc(a_hi + lay.a0_half, UM_A_LBO, A_SBO0) + h * A_HALF;
+          wg_fence();
+          ws_unroll<K0 / 8>([&](auto S) {
+            constexpr int s = decltype(S)::value, AO = s * A_STEP, WO = s * W_STEP;
+            wg_mma_n64_at<AO, WO>(d0, al, w0h_d, s > 0);  // small terms first
+            wg_mma_n64_at<AO, WO>(d0, ah, w0l_d, 1);
+            wg_mma_n64_at<AO, WO>(d0, ah, w0h_d, 1);
+          });
+          wg_commit();
+          wg_wait0();
+        }
+        __syncwarp();
+        if (lane == 0) ws_arrive(um_smem_u32(bars + WSB_A0_EMPTY + slot));  // the gather team may refill the A tile
+        clk.lap(1);
+        float o[2][4];
+        if (L > 1) {
+          // ---- layer-0 epilogue (the bias came through the MMA): gated activations -> layer 1 with the A operand
+          // from registers
+          float d1[32];
+          gate(d0, nullptr, bsel, true);
+          mma_rs64(d0, d1, w1h_d, w1l_d);
+          clk.lap(2);
+          // ---- last hidden layer: bias, gate, output head(s), results
+          gate(d1, s_b1, bsel, true);
+          head(d1, o);
+          store(T, i, o);
+        } else {
+          // single hidden layer: its bias came through the MMA
+          gate(d0, nullptr, bsel, true);
+          head(d0, o);
+          store(T, i, o);
+        }
+        clk.lap(3);
+      }
     }
   } else {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(WS_REG_G));
@@ -440,7 +596,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
     const int sub = lane / M::LPR, c4 = lane % M::LPR;
     const float4* __restrict__ f4 = reinterpret_cast<const float4*>(p.feat) + c4;
     constexpr int GU = NPASS / WS_GW >= 2 ? 2 : 1;  // passes in flight per gather warp
-    static_assert(MB % (WS_GT * BPT) == 0, "the slots of a team's meta blocks repeat every MB blocks");
+    static_assert(MB % (WS_GT * (GRAD ? WS_QG / WT : 128 / WT)) == 0, "the slots of a team's meta blocks repeat every MB blocks");
     constexpr int MD = MB / WS_GT;  // meta slots per team
     constexpr int PF = MD - 2;      // meta blocks in flight ahead of the one being gathered
     static_assert(PF >= 1, "meta ring too small to refill ahead");
@@ -462,7 +618,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
           ws_bulk_g2s(mt, p.stash + (size_t)st * StashS::floats, B_S, full);  // li | w | pos | perm: one copy
           if (GRAD) ws_bulk_g2s(mt + WsMeta::om, p.seeds + (size_t)st * Seeds::floats, B_SD, full);
         }
-      } else {  // tail of the last value-only tile: a block without neighbours
+      } else {  // tail of the last value-only tile or adjoint group: a block without neighbours
         for (int e = lane; e < MSTRIDE; e += 32) mt[e] = e < WsMeta::w ? __int_as_float(-1) : 0.f;
         __syncwarp();
         if (lane == 0) ws_arrive(full);
@@ -480,6 +636,20 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       const int slot = i % WS_A0;
       unsigned char* a_hi = sm + lay.a0 + slot * lay.a0_stride;
       unsigned char* a_lo = a_hi + lay.a0_half;
+      // chunk ch (columns 4 ch .. 4 ch + 3) of the row of type tt (0 value, 1..3 d/dq_{tt-1}) of query ql of meta
+      // block b: a forward-mode tile interleaves the four rows of a query and stores hi / lo TF32 parts, an adjoint
+      // group keeps fp32 blocks V, T1, T2, T3
+      auto put = [&](int b, int ql, int tt, int ch, float4 v) {
+        if (adj) {
+          *reinterpret_cast<float4*>(a_hi + ((tt * WS_QG + b * WT + ql) * WS_LDA + 4 * ch) * 4) = v;
+        } else {
+          float4 hi, lo;
+          um_split4(v, hi, lo);
+          const int off = um_a_off(GRAD ? 4 * ql + tt : b * WT + ql, ch, K0);
+          *reinterpret_cast<float4*>(a_hi + off) = hi;
+          *reinterpret_cast<float4*>(a_lo + off) = lo;
+        }
+      };
       bool slot_free = false;
 #pragma unroll 1
       for (int b = 0; b < BPT; ++b, ++j) {
@@ -540,20 +710,10 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
                   }
                 }
               }
-            const int row = GRAD ? 4 * ql : b * WT + ql;
-            float4 hi, lo;
-            um_split4(acc, hi, lo);
-            int off = um_a_off(row, c4, K0);
-            *reinterpret_cast<float4*>(a_hi + off) = hi;
-            *reinterpret_cast<float4*>(a_lo + off) = lo;
+            put(b, ql, 0, c4, acc);
             if (GRAD) {
 #pragma unroll
-              for (int j = 0; j < 3; ++j) {
-                um_split4(tq[j], hi, lo);
-                off = um_a_off(row + 1 + j, c4, K0);
-                *reinterpret_cast<float4*>(a_hi + off) = hi;
-                *reinterpret_cast<float4*>(a_lo + off) = lo;
-              }
+              for (int j = 0; j < 3; ++j) put(b, ql, 1 + j, c4, tq[j]);
             }
           }
           clk.lap(3);
@@ -567,20 +727,15 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
           reinterpret_cast<int*>(sm + lay.qidx)[(i % WS_QX) * QT + b * WT + lane] = reinterpret_cast<const int*>(mt + WsMeta::perm)[lane];
         // position part (columns F .. F+2) and zero padding of the rows: thread per row
         if (GRAD || (b % WS_GW) == gw) {
-          const int row = GRAD ? gw * WT + lane : b * WT + lane;
-          const int ql = GRAD ? row >> 2 : lane, tt = GRAD ? row & 3 : 0;
+          const int row = gw * WT + lane;  // forward mode: row of the tile
+          const int ql = adj ? lane : (GRAD ? row >> 2 : lane), tt = adj ? gw : (GRAD ? row & 3 : 0);
           const float* src3 = tt == 0 ? mt + WsMeta::xn : mt + WsMeta::P + (tt - 1) * 3 * WT;
-          float4 hi, lo;
-          um_split4(make_float4(src3[ql], src3[WT + ql], src3[2 * WT + ql], tt == 0 ? 1.f : 0.f), hi, lo);  // column D: bias input
-          int off = um_a_off(row, F / 4, K0);
-          *reinterpret_cast<float4*>(a_hi + off) = hi;
-          *reinterpret_cast<float4*>(a_lo + off) = lo;
+          put(b, ql, tt, F / 4, make_float4(src3[ql], src3[WT + ql], src3[2 * WT + ql], tt == 0 ? 1.f : 0.f));  // column D: bias input
+          // columns an adjoint group does not store (>= WS_LDA) are zero in the consumers' registers
+          const int n_ch = adj ? (K0 < WS_LDA ? K0 : WS_LDA) / 4 : K0 / 4;
 #pragma unroll
-          for (int cz = F / 4 + 1; cz < K0 / 4; ++cz) {
-            off = um_a_off(row, cz, K0);
-            *reinterpret_cast<float4*>(a_hi + off) = make_float4(0.f, 0.f, 0.f, 0.f);
-            *reinterpret_cast<float4*>(a_lo + off) = make_float4(0.f, 0.f, 0.f, 0.f);
-          }
+          for (int cz = F / 4 + 1; cz < K0 / 4; ++cz)
+            if (cz < n_ch) put(b, ql, tt, cz, make_float4(0.f, 0.f, 0.f, 0.f));
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // A-tile writes -> visible to wgmma
         __syncwarp();
@@ -590,7 +745,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       if (lane == 0) ws_arrive(um_smem_u32(bars + WSB_A0_FULL + slot));
     }
   }
-  clk.flush(warp, warp < WS_CW ? WS_ROLE_C : WS_ROLE_G);
+  clk.flush(warp, warp < WS_CW ? (adj ? WS_ROLE_CA : WS_ROLE_C) : WS_ROLE_G);
 }
 
 // ---------------------------------------------------------------------------
@@ -607,18 +762,25 @@ static WsLayout plan_ws_layout(const pinb200_decoder_view& d, bool grad) {
     return at;
   };
   const int w0 = 64 * DM::K0 * 4, w1 = 64 * 64 * 4;
+  // d/dq of a single output channel takes the adjoint schedule; a colour Jacobian (out_dim 3) would need one adjoint
+  // vector per channel and saves no MMA work, so it stays in forward mode
+  l.adj = grad && d.out_dim == 1;
   l.w0_hi = take(w0);
   l.w0_lo = take(w0);
   if (d.n_hidden > 1) {
     l.w1_hi = take(w1);
     l.w1_lo = take(w1);
+    if (l.adj) {
+      l.w1t_hi = take(w1);
+      l.w1t_lo = take(w1);
+    }
   }
   l.b0 = take(64 * 4);
   l.b1 = take(64 * 4);
   l.wout = take(4 * 64 * 4);
   l.bout = take(16);
   l.a0_half = ((UM_ROWS / 8) * (DM::K0 / 4) * UM_A_LBO + 127) & ~127;
-  l.a0_stride = 2 * l.a0_half;
+  l.a0_stride = l.adj ? 4 * WS_GBLK * 4 : 2 * l.a0_half;
   l.a0 = take(WS_A0 * l.a0_stride);
   l.qidx = take(WS_QX * 128 * 4);
   l.meta_stride = (grad ? WsMeta::floats_g : WsMeta::floats_ng) * 4;
@@ -641,7 +803,7 @@ static int launch_wsq(QueryParams& p, cudaStream_t stream) {
   if (const int rc = prepare_kernel((const void*)kern, "wsq_decode_kernel", smem_bytes)) return rc;
   p.qpt = WT;
   p.n_tiles = (int)((p.n + WT - 1) / WT);
-  constexpr int QT = GRAD ? 32 : 128;
+  const int QT = lay.adj ? WS_QG : (GRAD ? 32 : 128);
   const long long n_tiles = (p.n + QT - 1) / QT;
   const int grid = (int)std::min<long long>(n_tiles, (long long)sm_count());
   cudaLaunchConfig_t cfg{};

@@ -136,6 +136,7 @@ if args.sort_sweep:
 # role codes as written by wsq.cu (WS_ROLE_*) -> (name, slot names, indices of the slots that are waits)
 ROLES = {
     1: ("C consumer", ["wait_A", "layer0", "layer1", "last+out"], {0}),
+    2: ("C consumer, adjoint schedule", ["wait_A", "value_rows", "adjoint", "tangents+out"], {0}),
     4: ("G gather + meta refill", ["wait_A_free", "wait_meta", "issue_loads", "reduce+store", "pos+fence",
                                    "meta_refill", "wait_search"], {0, 1, 6}),
 }

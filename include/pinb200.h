@@ -338,6 +338,10 @@ typedef struct pinb200_map_train_opts {
   void* nccl_comm;    /* from pinb200_nccl_init, or NULL */
   float* reduce_buf;
   int64_t reduce_count;
+  /* scratch of the training forward (pinb200_query_opts.workspace): with >= pinb200_query_workspace_bytes(rows)
+   * bytes, batches of at least PINB200_SPLIT_MIN_QUERIES rows run as two launches like any other query; NULL: one */
+  void* workspace;
+  int64_t workspace_bytes;
 } pinb200_map_train_opts;
 
 /* n_iter x [assemble_batch -> query_sdf(training) -> mapping_loss -> train_backward -> adam(decoder) -> adam(features)].

@@ -66,7 +66,8 @@ class MapTrainOpts(C.Structure):
                 ("ts", c_i32p), ("weight", c_f32p), ("dloss", c_f32p), ("losses", c_f32p), ("feat", c_f32p),
                 ("dec_flat", c_f32p), ("grad_feat", c_f32p), ("grad_dec", c_f32p), ("m_feat", c_f32p),
                 ("v_feat", c_f32p), ("m_dec", c_f32p), ("v_dec", c_f32p), ("nccl_comm", C.c_void_p),
-                ("reduce_buf", c_f32p), ("reduce_count", C.c_int64)]
+                ("reduce_buf", c_f32p), ("reduce_count", C.c_int64), ("workspace", C.c_void_p),
+                ("workspace_bytes", C.c_int64)]
 
 
 # name -> (restype, argtypes); every symbol include/pinb200.h declares

@@ -238,6 +238,8 @@ extern "C" int pinb200_map_iterations(const pinb200_map_view* map, const pinb200
   qo.need_grad = 0;
   qo.training_rows = n;
   qo.transform = nullptr;
+  qo.workspace = t->workspace;
+  qo.workspace_bytes = t->workspace_bytes;
   const bool do_fb = (t->stages & 1) != 0, do_opt = (t->stages & 2) != 0;
   for (int it = 0; it < n_iter; ++it) {
     int rc = PINB200_OK;

@@ -439,7 +439,7 @@ def map_iterations(mh: MapHandle, dec: DecoderHandle, n_iter: int, *, nn_k, weig
         return t
 
     rows_t = buf("rows", (rows, 3))
-    _, qo, _ = _query_args(rows_t, nn_k, weighted_first, True, False, None, False, None, True, False, bs, work)
+    _, qo, qopts = _query_args(rows_t, nn_k, weighted_first, True, False, None, False, None, True, False, bs, work)
     t = MapTrainOpts()
     t.coord_pool, t.label_pool = _ptr(coord_pool, torch.float32), _ptr(label_pool, torch.float32)
     t.ts_pool, t.weight_pool = _ptr(ts_pool, torch.int32), _ptr(weight_pool, torch.float32)
@@ -448,6 +448,7 @@ def map_iterations(mh: MapHandle, dec: DecoderHandle, n_iter: int, *, nn_k, weig
     t.lr, t.beta1, t.beta2, t.eps, t.weight_decay = float(lr), float(beta1), float(beta2), float(eps), float(weight_decay)
     t.train_decoder, t.first_step = int(bool(train_decoder)), int(first_step)
     t.stages, t.grad_scale = int(stages), float(grad_scale)
+    t.workspace, t.workspace_bytes = qopts.workspace, qopts.workspace_bytes  # the split training forward's scratch
     t.rows = _ptr(rows_t)
     t.label, t.ts, t.weight = _ptr(buf("label", (bs,))), _ptr(buf("ts", (bs,), torch.int32)), _ptr(buf("weight", (bs,)))
     t.dloss, t.losses = _ptr(buf("dl", (rows,))), _ptr(losses, torch.float32)

@@ -50,11 +50,9 @@ constexpr int WS_THREADS = (WS_CW + WS_GT * WS_GW) * 32;
 // (512 threads x 128 registers)
 constexpr int WS_REG_C = 136, WS_REG_G = 120;
 static_assert((WS_CW * WS_REG_C + WS_GT * WS_GW * WS_REG_G) * 32 <= WS_THREADS * 128, "setmaxnreg pool");
-constexpr int WS_A0 = 2;       // A-tile ring slots, one per gather team
-// ring of the original query indices of a tile: tile i in slot i % WS_QX.  Slot i % WS_QX is
-// rewritten for tile i + WS_QX only after the A tile of tile i + WS_A0 was released, i.e. after every consumer warp
-// stored tile i
-constexpr int WS_QX = 2 * WS_A0;
+// A-tile ring slots: 2 (one per gather team) in forward mode and value-only; the adjoint schedule takes the most that
+// fit next to its weights (plan_ws_layout), so that a team gathers its next group while its warpgroup decodes
+constexpr int WS_A0_MAX = 4;
 // adjoint schedule (d/dq of a single-output head): a group of 64 queries is four 64-row fp32 blocks V, T1, T2, T3 of
 // WS_LDA floats per row; WS_LDA == 4 (mod 32) keeps the consumers' scalar A-fragment loads free of bank conflicts.
 // Columns >= WS_LDA (the last four of K0 = 40) are zero and never stored
@@ -77,14 +75,51 @@ struct WsLayout {  // byte offsets from the dynamic shared memory base
   int adj;                     // 1: adjoint schedule (d/dq with one output channel), A slots are fp32 groups
   int w0_hi, w0_lo, w1_hi, w1_lo, w1t_hi, w1t_lo, b0, b1, wout, bout;
   int a0, a0_half, a0_stride;  // ring of A tiles: slot s = [a0 + s*stride: hi | + half: lo] (adjoint: one fp32 group)
-  int qidx;                    // [WS_QX][128] original query index of every tile row's query
+  int n_slots, a0_period, a0_cycle;  // S, slots of the A ring, P = lcm(S, 2) and 2P (WsRing)
+  // [n_qx][128] original query index of every tile row's query, tile i in slot i % n_qx.  The filler of tile i + n_qx
+  // writes that slot after the release of tile i + n_qx - S.  Forward mode (S = 2, n_qx = 2P = 4, slot i mod 2P): a
+  // release comes after layer 0, so tile i + S released means every consumer warp has stored tile i.  Adjoint
+  // (n_qx = S, slot i % S): a consumer warp reads its query indices before it releases group i
+  int qidx, n_qx;
   int meta, meta_stride, n_meta;
   int bars, total;
 };
-// mbarrier indices
+// mbarrier indices: FULL[slot][i % 2] and EMPTY[slot][i % 2] of the A ring (WsRing), then the meta ring's
 constexpr int WS_MB_MAX = 16;
-constexpr int WSB_A0_FULL = 0, WSB_A0_EMPTY = WSB_A0_FULL + WS_A0, WSB_META_FULL = WSB_A0_EMPTY + WS_A0,
+constexpr int WSB_A0_FULL = 0, WSB_A0_EMPTY = WSB_A0_FULL + 2 * WS_A0_MAX, WSB_META_FULL = WSB_A0_EMPTY + 2 * WS_A0_MAX,
               WSB_META_EMPTY = WSB_META_FULL + WS_MB_MAX, WSB_COUNT = WSB_META_EMPTY + WS_MB_MAX;
+
+// The A ring.  Tile (adjoint: group) i of a CTA lives in slot s = i % S and is filled by gather team i % 2; in the
+// adjoint schedule warpgroup i % 2 alone decodes it.  The slot's previous user is tile i - S, which belongs to the
+// other team when S is odd, so the barriers are keyed by (slot, i % 2): FULL[s][i % 2] completes a phase when tile i
+// is filled and EMPTY[s][i % 2] when it is released.  With P = lcm(S, 2) the tiles on one barrier are i, i + P, ...,
+// so tile i is phase i / P of both.  A parity wait is exact when the waiter has seen the phase before the one it waits
+// for, and the barrier cannot complete the phase after it first:
+//  * the consumer of tile i waits for phase i / P of FULL[s][i % 2].  It consumed tile i - P, the phase before, itself.
+//    The fill of tile i + P waits for the release of tile i + P - S (S even: tile i; S = 3: tile i + 3, whose fill
+//    waits for the release of tile i), so it comes after this consumer releases tile i.
+//  * the filler of tile i waits for the release of tile i - S: phase (i - S) / P of EMPTY[s][(i - S) % 2] (for i < S
+//    the parity of phase -1, which a fresh barrier passes).  Its team waited for the phase before when it filled tile
+//    i - P.  The release of tile i - S + P needs that tile filled, which comes after the fill of tile i (S even: it is
+//    tile i; S = 3: it waits for the release of tile i).
+// The same chains order every arrival on a phase after the completion of the phase before.  One barrier per slot
+// would not do for S = 3: the consumer of tile i + 6 could pass on the parity of the fill of tile i + 3.
+// The helpers take k = i mod 2P, which the loops step along with i: compares instead of divisions by the run-time S
+// and P (whose reciprocals would stay live in registers across the consumers' loop).
+struct WsRing {
+  int S, P, P2;  // S, P and 2P from the launch's plan, so that they stay kernel-parameter operands
+  __device__ __forceinline__ int next(int k, int step) const { return k + step >= P2 ? k + step - P2 : k + step; }
+  __device__ __forceinline__ int slot(int k) const {
+    const int r = k >= P ? k - P : k;  // i mod P, and P <= 2 S
+    return r >= S ? r - S : r;
+  }
+  __device__ __forceinline__ uint32_t parity(int k) const { return k >= P ? 1u : 0u; }  // of phase i / P
+  __device__ __forceinline__ int full(int k) const { return WSB_A0_FULL + 2 * slot(k) + (k & 1); }
+  __device__ __forceinline__ int empty(int k) const { return WSB_A0_EMPTY + 2 * slot(k) + (k & 1); }
+  // what the filler of tile i waits on: the release of tile i - S.  For i < S, (i - S) mod 2P >= P: phase -1 is odd
+  __device__ __forceinline__ int prev_empty(int k) const { return WSB_A0_EMPTY + 2 * slot(k) + ((k + S) & 1); }
+  __device__ __forceinline__ uint32_t prev_parity(int k) const { return parity(k >= S ? k - S : k - S + P2); }
+};
 
 // Optional cycle accounting (pinb200_set_option("ws_profile", 1)): per warp, clock deltas of up to 7 phases,
 // summed over the tiles of the launch, for the first WS_PROF_CTAS CTAs; read back with
@@ -207,7 +242,9 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
   const bool adj = GRAD && lay.adj;     // adjoint schedule: tiles are 64-query groups, one per consumer warpgroup
   const int QT = adj ? WS_QG : (GRAD ? 32 : 128);  // queries per tile
   const int BPT = QT / WT;              // meta blocks per tile
-  constexpr int MB = GRAD ? 8 : 16;     // meta ring slots (blocks of 32 queries; a value-only tile has 4)
+  const int MB = lay.n_meta;            // meta ring slots (blocks of 32 queries; a value-only tile has 4), a power of 2:
+                                        // block blk is in slot blk & (MB - 1), phase parity blk & MB
+  const WsRing ring{lay.n_slots, lay.a0_period, lay.a0_cycle};
   constexpr int MSTRIDE = GRAD ? WsMeta::floats_g : WsMeta::floats_ng;
   constexpr int NPASS = WT / M::RPP;    // gather passes per meta block (F = 32: 8 passes of 4 queries)
   extern __shared__ __align__(1024) unsigned char ws_smem[];
@@ -225,7 +262,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
     auto init = [&](int i, int count) {
       asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(um_smem_u32(bars + i)), "r"(count));
     };
-    for (int s = 0; s < WS_A0; ++s) {
+    for (int s = 0; s < 2 * WS_A0_MAX; ++s) {
       init(WSB_A0_FULL + s, WS_GW);
       init(WSB_A0_EMPTY + s, adj ? 4 : WS_CW);  // adjoint: one warpgroup consumes a group
     }
@@ -366,9 +403,9 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
     }
     // value rows write the prediction, tangent rows one component of its gradient; lane c == r of the quad writes row r.
     // Tile i holds queries T * QT .. in search order, mapped to their original index through the index ring the
-    // gather team filled (shared memory: no global load on this path)
+    // gather team filled (shared memory: no global load on this path), in slot rk = i mod 2P
     const int* s_qidx = reinterpret_cast<const int*>(sm + lay.qidx);
-    auto store = [&](long long T, int i, float (&o)[2][4]) {
+    auto store = [&](long long T, int rk, float (&o)[2][4]) {
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         if (p.dec.sigmoid_out) {
@@ -387,7 +424,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
         }
         const int row = 64 * h + 16 * wq + g8 + 8 * r, qrow = GRAD ? (row >> 2) : row;
         if (c == r && T * QT + qrow < p.n) {  // the tail of the last tile carries no valid index
-          const long long qi = s_qidx[(i % WS_QX) * QT + qrow];
+          const long long qi = s_qidx[rk * QT + qrow];
           if (out_base) {
             float* dst = out_base + qi * out_qstride;
 #pragma unroll
@@ -402,7 +439,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
     if (adj) {
       // ---------------------------------------------------------------------------------------------------
       // Adjoint schedule (d/dq of a single-output head): warpgroup h consumes the groups i = h (mod 2) of this CTA,
-      // which gather team h fills into A slot h.  Row r of each block V, T1, T2, T3 of a group is query r, so the
+      // which gather team h fills into A slot i % S.  Row r of each block V, T1, T2, T3 of a group is query r, so the
       // thread that holds element (r, col) of u_j = W0 T_j also holds it for the value rows and for
       //   v' = D0 W1^T (w_out . D1)   (L = 1: D0 w_out),   and   d out / d q_j = v' . u_j:
       // the tangents stop at layer 0 and need neither the value row's mask shuffle nor a second layer.
@@ -415,8 +452,9 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       float* out_g = p.is_color ? p.out.color_grad : p.out.grad;
       float* out_s = p.is_color ? nullptr : p.out.sdf_std;
       // layer 0 of one 64-row block: the A fragments come from the fp32 group and are split into hi / lo in registers
-      // (same 3xTF32 terms and order as an A tile stored hi / lo).  `release` frees the A slot once they are loaded
-      auto layer0 = [&](const float* blk, float (&d)[32], int slot, bool release) {
+      // (same 3xTF32 terms and order as an A tile stored hi / lo).  `release` arrives on the A-slot barrier `empty`
+      // once they are loaded
+      auto layer0 = [&](const float* blk, float (&d)[32], uint32_t empty, bool release) {
         const float* r = blk + row0 * WS_LDA + c;
         float a[K0 / 8][4];
         ws_unroll<K0 / 8>([&](auto S) {
@@ -432,7 +470,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
         });
         if (release) {
           __syncwarp();
-          if (lane == 0) ws_arrive(um_smem_u32(bars + WSB_A0_EMPTY + slot));  // the gather team may refill the slot
+          if (lane == 0) ws_arrive(empty);  // a gather team may refill the slot
         }
 #pragma unroll
         for (int e = 0; e < 32; ++e) d[e] = 0.f;
@@ -453,15 +491,16 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
         wg_wait0();
       };
 
-      int i = h;
-      for (long long G = blockIdx.x + (long long)h * gridDim.x; G < n_tiles; G += (long long)WS_GT * gridDim.x, i += WS_GT) {
-        const int slot = i % WS_A0;
-        ws_wait(um_smem_u32(bars + WSB_A0_FULL + slot), (uint32_t)(i / WS_A0) & 1u);
+      int rk = h;  // group i = h, h + 2, ... of this CTA; rk = i mod 2P
+      for (long long G = blockIdx.x + (long long)h * gridDim.x; G < n_tiles; G += (long long)WS_GT * gridDim.x, rk = ring.next(rk, WS_GT)) {
+        const int slot = ring.slot(rk);
+        ws_wait(um_smem_u32(bars + ring.full(rk)), ring.parity(rk));
         clk.lap(0);
         const float* grp = reinterpret_cast<const float*>(sm + lay.a0 + slot * lay.a0_stride);
+        const uint32_t empty = um_smem_u32(bars + ring.empty(rk));
         // ---- value rows: layer 0 (bias through the MMA), gate, layer 1, head, sdf
         float d0[32], v[32], o[2][4];
-        layer0(grp, d0, slot, false);
+        layer0(grp, d0, empty, false);
         const uint32_t m0 = gate(d0, nullptr, 1.f, false);
         if (L > 1) {
           mma_rs64(d0, v, w1h_d, w1l_d);
@@ -478,7 +517,8 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
         }
         // lane c = r of a quad stores the results of row r (r = 0, 1)
         const bool st = c < 2 && G * QT + row0 + 8 * c < p.n;  // the tail of the last group carries no valid index
-        const long long qi = st ? s_qidx[(i % WS_QX) * QT + row0 + 8 * c] : 0;
+        // the query-index ring has one slot per A slot here (n_qx = S); read before the A slot is released
+        const long long qi = st ? s_qidx[slot * QT + row0 + 8 * c] : 0;
         float sc[2];  // d out / d (head sum) of the two rows
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
@@ -510,7 +550,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
         float* const gdst = st && out_g ? out_g + 3 * qi : nullptr;
 #pragma unroll
         for (int j = 0; j < 3; ++j) {
-          layer0(grp + (j + 1) * WS_GBLK, d0, slot, j == 2);
+          layer0(grp + (j + 1) * WS_GBLK, d0, empty, j == 2);
           float g[2];
 #pragma unroll
           for (int r = 0; r < 2; ++r) {
@@ -528,17 +568,16 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
         clk.lap(3);
       }
     } else {
-      int i = 0;
-      for (long long T = blockIdx.x; T < n_tiles; T += gridDim.x, ++i) {
-        const int slot = i % WS_A0;
-        ws_wait(um_smem_u32(bars + WSB_A0_FULL + slot), (uint32_t)(i / WS_A0) & 1u);
+      int rk = 0;  // tile i = 0, 1, ... of this CTA; rk = i mod 2P
+      for (long long T = blockIdx.x; T < n_tiles; T += gridDim.x, rk = ring.next(rk, 1)) {
+        ws_wait(um_smem_u32(bars + ring.full(rk)), ring.parity(rk));
         clk.lap(0);
         // ---- layer 0 of this warpgroup's half, A tile from shared memory
         float d0[32];
 #pragma unroll
         for (int e = 0; e < 32; ++e) d0[e] = 0.f;
         {
-          const uint32_t a_hi = um_smem_u32(sm + lay.a0 + slot * lay.a0_stride);
+          const uint32_t a_hi = um_smem_u32(sm + lay.a0 + ring.slot(rk) * lay.a0_stride);
           const uint64_t ah = um_desc(a_hi, UM_A_LBO, A_SBO0) + h * A_HALF, al = um_desc(a_hi + lay.a0_half, UM_A_LBO, A_SBO0) + h * A_HALF;
           wg_fence();
           ws_unroll<K0 / 8>([&](auto S) {
@@ -551,7 +590,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
           wg_wait0();
         }
         __syncwarp();
-        if (lane == 0) ws_arrive(um_smem_u32(bars + WSB_A0_EMPTY + slot));  // the gather team may refill the A tile
+        if (lane == 0) ws_arrive(um_smem_u32(bars + ring.empty(rk)));  // a gather team may refill the A tile
         clk.lap(1);
         float o[2][4];
         if (L > 1) {
@@ -564,12 +603,12 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
           // ---- last hidden layer: bias, gate, output head(s), results
           gate(d1, s_b1, bsel, true);
           head(d1, o);
-          store(T, i, o);
+          store(T, rk, o);
         } else {
           // single hidden layer: its bias came through the MMA
           gate(d0, nullptr, bsel, true);
           head(d0, o);
-          store(T, i, o);
+          store(T, rk, o);
         }
         clk.lap(3);
       }
@@ -585,10 +624,12 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
     // The teams also fill the meta ring: TMA bulk copies (cp.async.bulk, completion counted in bytes on the block's
     // "full" mbarrier; no thread touches the data) of what search_kernel wrote for a 32-query block -- the StashS block
     // (2.5 KB: neighbour ids, IDW weights, position part, original query indices) and, with d/dq, the forward-mode
-    // seeds (4.1 KB).  Block blk + MB of the
-    // ring belongs to the same team as block blk, so a team refills its own slots: position j of the team's stream of
-    // meta blocks takes the slot of position j - MD, and before it works on position j one warp of the team (in
-    // turn) issues position j + PF, whose slot the team left two positions ago.
+    // seeds (4.1 KB).  Block blk + MB of the ring belongs to the same team as block blk (plan_ws_layout checks that
+    // MB is a multiple of 2 tiles), so a team refills its own slots: position j of the team's stream of meta blocks
+    // takes the slot of position j - MD, and before it works on position j one warp of the team (in turn) issues
+    // position j + PF, whose slot the team left two positions ago.  A team ring of two blocks (MD = 2, one adjoint
+    // group) issues one position ahead, into the slot of position j - 1: that refill waits until the team's last
+    // warp has left it, and the copies have the gather time of one block to land.
     // profile slots: 0 wait free A tile, 1 wait meta block, 2 feature-row loads issued, 3 reduce + A-tile stores,
     //                4 position rows + fence + arrive, 5 meta refill (wait free slot + copies), 6 wait for the search grid
     // =====================================================================================================
@@ -596,18 +637,16 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
     const int sub = lane / M::LPR, c4 = lane % M::LPR;
     const float4* __restrict__ f4 = reinterpret_cast<const float4*>(p.feat) + c4;
     constexpr int GU = NPASS / WS_GW >= 2 ? 2 : 1;  // passes in flight per gather warp
-    static_assert(MB % (WS_GT * (GRAD ? WS_QG / WT : 128 / WT)) == 0, "the slots of a team's meta blocks repeat every MB blocks");
-    constexpr int MD = MB / WS_GT;  // meta slots per team
-    constexpr int PF = MD - 2;      // meta blocks in flight ahead of the one being gathered
-    static_assert(PF >= 1, "meta ring too small to refill ahead");
+    const int MD = MB / WS_GT;              // meta slots per team
+    const int PF = MD > 2 ? MD - 2 : 1;     // meta blocks in flight ahead of the one being gathered
     // position jj of this team's stream: block b = jj % BPT of its tile i = team + WS_GT * (jj / BPT)
     auto refill = [&](int jj) {
       if (jj % WS_GW != gw) return;
       const int ri = team + WS_GT * (jj / BPT), b = jj % BPT;
       const long long T = blockIdx.x + (long long)ri * gridDim.x;
       if (T >= n_tiles) return;
-      const int blk = ri * BPT + b, ms = blk % MB;
-      ws_wait_relaxed(um_smem_u32(bars + WSB_META_EMPTY + ms), ((uint32_t)(blk / MB) & 1u) ^ 1u);
+      const int blk = ri * BPT + b, ms = blk & (MB - 1);
+      ws_wait_relaxed(um_smem_u32(bars + WSB_META_EMPTY + ms), (blk & MB) ? 0u : 1u);
       float* mt = meta + ms * MSTRIDE;
       const uint32_t full = um_smem_u32(bars + WSB_META_FULL + ms);
       const long long st = T * BPT + b;  // stash block
@@ -631,10 +670,10 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
     clk.lap(6);
     for (int jj = 0; jj < PF; ++jj) refill(jj);
     clk.lap(5);
-    int i = team, j = 0;
-    for (long long T = blockIdx.x + (long long)team * gridDim.x; T < n_tiles; T += (long long)WS_GT * gridDim.x, i += WS_GT) {
-      const int slot = i % WS_A0;
-      unsigned char* a_hi = sm + lay.a0 + slot * lay.a0_stride;
+    int i = team, rk = team, j = 0;  // rk = i mod 2P
+    for (long long T = blockIdx.x + (long long)team * gridDim.x; T < n_tiles;
+         T += (long long)WS_GT * gridDim.x, i += WS_GT, rk = ring.next(rk, WS_GT)) {
+      unsigned char* a_hi = sm + lay.a0 + ring.slot(rk) * lay.a0_stride;
       unsigned char* a_lo = a_hi + lay.a0_half;
       // chunk ch (columns 4 ch .. 4 ch + 3) of the row of type tt (0 value, 1..3 d/dq_{tt-1}) of query ql of meta
       // block b: a forward-mode tile interleaves the four rows of a query and stores hi / lo TF32 parts, an adjoint
@@ -655,8 +694,8 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
       for (int b = 0; b < BPT; ++b, ++j) {
         refill(j + PF);
         clk.lap(5);
-        const int blk = i * BPT + b, ms = blk % MB;
-        ws_wait_relaxed(um_smem_u32(bars + WSB_META_FULL + ms), (uint32_t)(blk / MB) & 1u);
+        const int blk = i * BPT + b, ms = blk & (MB - 1);
+        ws_wait_relaxed(um_smem_u32(bars + WSB_META_FULL + ms), (blk & MB) ? 1u : 0u);
         clk.lap(1);
         const float* mt = meta + ms * MSTRIDE;
         const int* m_li = reinterpret_cast<const int*>(mt + WsMeta::li);
@@ -678,7 +717,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
           }
           clk.lap(2);
           if (!slot_free) {  // the loads are in flight while the previous tile in this slot is consumed by layer 0
-            ws_wait_relaxed(um_smem_u32(bars + WSB_A0_EMPTY + slot), ((uint32_t)(i / WS_A0) & 1u) ^ 1u);
+            ws_wait_relaxed(um_smem_u32(bars + ring.prev_empty(rk)), ring.prev_parity(rk));
             slot_free = true;
             clk.lap(0);
           }
@@ -719,12 +758,12 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
           clk.lap(3);
         }
         if (!slot_free) {  // warps without a pass in this block (F = 8) still write position rows
-          ws_wait_relaxed(um_smem_u32(bars + WSB_A0_EMPTY + slot), ((uint32_t)(i / WS_A0) & 1u) ^ 1u);
+          ws_wait_relaxed(um_smem_u32(bars + ring.prev_empty(rk)), ring.prev_parity(rk));
           slot_free = true;
         }
         // the tile's original query indices, for the consumers' stores (the meta slot is refilled before they store)
         if ((b % WS_GW) == gw)
-          reinterpret_cast<int*>(sm + lay.qidx)[(i % WS_QX) * QT + b * WT + lane] = reinterpret_cast<const int*>(mt + WsMeta::perm)[lane];
+          reinterpret_cast<int*>(sm + lay.qidx)[(adj ? ring.slot(rk) : rk) * QT + b * WT + lane] = reinterpret_cast<const int*>(mt + WsMeta::perm)[lane];
         // position part (columns F .. F+2) and zero padding of the rows: thread per row
         if (GRAD || (b % WS_GW) == gw) {
           const int row = gw * WT + lane;  // forward mode: row of the tile
@@ -742,7 +781,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
         if (lane == 0) ws_arrive(um_smem_u32(bars + WSB_META_EMPTY + ms));
         clk.lap(4);
       }
-      if (lane == 0) ws_arrive(um_smem_u32(bars + WSB_A0_FULL + slot));
+      if (lane == 0) ws_arrive(um_smem_u32(bars + ring.full(rk)));
     }
   }
   clk.flush(warp, warp < WS_CW ? (adj ? WS_ROLE_CA : WS_ROLE_C) : WS_ROLE_G);
@@ -751,23 +790,24 @@ __global__ void __launch_bounds__(WS_THREADS, 1) wsq_decode_kernel(const __grid_
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
+constexpr int WS_SMEM_MAX = 227 * 1024;  // dynamic shared memory of one CTA on an H100
+
+// the layout of a launch with n_slots A slots and n_meta meta blocks
 template <int FT>
-static WsLayout plan_ws_layout(const pinb200_decoder_view& d, bool grad) {
+constexpr WsLayout ws_layout(int n_hidden, bool grad, bool adj, int n_slots, int n_meta) {
   using DM = UmmaDims<FT>;
   WsLayout l{};
   int o = 0;
-  auto take = [&](int bytes) {
+  auto take = [&o](int bytes) {
     const int at = o;
     o += (bytes + 127) & ~127;
     return at;
   };
   const int w0 = 64 * DM::K0 * 4, w1 = 64 * 64 * 4;
-  // d/dq of a single output channel takes the adjoint schedule; a colour Jacobian (out_dim 3) would need one adjoint
-  // vector per channel and saves no MMA work, so it stays in forward mode
-  l.adj = grad && d.out_dim == 1;
+  l.adj = adj;
   l.w0_hi = take(w0);
   l.w0_lo = take(w0);
-  if (d.n_hidden > 1) {
+  if (n_hidden > 1) {
     l.w1_hi = take(w1);
     l.w1_lo = take(w1);
     if (l.adj) {
@@ -781,21 +821,69 @@ static WsLayout plan_ws_layout(const pinb200_decoder_view& d, bool grad) {
   l.bout = take(16);
   l.a0_half = ((UM_ROWS / 8) * (DM::K0 / 4) * UM_A_LBO + 127) & ~127;
   l.a0_stride = l.adj ? 4 * WS_GBLK * 4 : 2 * l.a0_half;
-  l.a0 = take(WS_A0 * l.a0_stride);
-  l.qidx = take(WS_QX * 128 * 4);
+  l.n_slots = n_slots;
+  l.a0_period = n_slots % 2 ? 2 * n_slots : n_slots;
+  l.a0_cycle = 2 * l.a0_period;
+  l.a0 = take(n_slots * l.a0_stride);
+  l.n_qx = adj ? n_slots : 2 * l.a0_period;
+  l.qidx = take(l.n_qx * 128 * 4);
   l.meta_stride = (grad ? WsMeta::floats_g : WsMeta::floats_ng) * 4;
-  l.n_meta = grad ? 8 : 16;
+  l.n_meta = n_meta;
   l.meta = take(l.n_meta * l.meta_stride);
   l.bars = take(WSB_COUNT * 8);
   l.total = o;
   return l;
 }
 
+// d/dq of a single output channel takes the adjoint schedule; a colour Jacobian (out_dim 3) would need one adjoint
+// vector per channel and saves no MMA work, so it stays in forward mode.  Forward mode and value-only launches keep
+// two A slots and a meta ring of 8 (16) blocks.  The adjoint schedule holds a group's slot for its whole decode, so
+// it takes the most slots S in {2, 3, 4} that fit, then a meta ring of 8 blocks if it still fits, otherwise 4 (one
+// group per team)
+template <int FT>
+constexpr WsLayout plan_ws_layout(int n_hidden, int out_dim, bool grad) {
+  const bool adj = grad && out_dim == 1;
+  if (!adj) return ws_layout<FT>(n_hidden, grad, false, 2, grad ? 8 : 16);
+  for (int s = WS_A0_MAX; s >= 2; --s)
+    for (int mb = 8; mb >= 4; mb -= 4) {
+      const WsLayout l = ws_layout<FT>(n_hidden, true, true, s, mb);
+      if (l.total <= WS_SMEM_MAX) return l;
+    }
+  return ws_layout<FT>(n_hidden, true, true, 2, 4);  // too large: the launcher reports it
+}
+
+// every decoder shape the kernel takes fits, and the meta slots of a team repeat every n_meta blocks (n_meta is a
+// multiple of two tiles' blocks, and a power of two)
+template <int FT>
+constexpr bool ws_plans_fit() {
+  for (int L = 1; L <= 2; ++L)
+    for (int oc = 1; oc <= 4; ++oc)
+      for (int g = 0; g < 2; ++g) {
+        const WsLayout l = plan_ws_layout<FT>(L, oc, g != 0);
+        const int bpt = (l.adj ? WS_QG : (g ? 32 : 128)) / WT;
+        if (l.total > WS_SMEM_MAX || l.n_meta % (WS_GT * bpt) != 0 || (l.n_meta & (l.n_meta - 1)) != 0 ||
+            l.n_meta > WS_MB_MAX || l.n_slots > WS_A0_MAX)
+          return false;
+        if (!l.adj && (l.n_slots != 2 || l.n_meta != (g ? 8 : 16))) return false;
+      }
+  return true;
+}
+static_assert(ws_plans_fit<8>() && ws_plans_fit<16>() && ws_plans_fit<32>(), "a wsq_decode_kernel layout does not fit");
+// the adjoint schedule: two-layer heads get 3 A slots next to W1^T with a 4-block meta ring, one-layer heads 4 slots
+template <int FT>
+constexpr bool ws_adjoint_plan(int L, int slots, int n_meta) {
+  return plan_ws_layout<FT>(L, 1, true).n_slots == slots && plan_ws_layout<FT>(L, 1, true).n_meta == n_meta;
+}
+static_assert(ws_adjoint_plan<8>(2, 3, 4) && ws_adjoint_plan<16>(2, 3, 4) && ws_adjoint_plan<32>(2, 3, 4),
+              "adjoint plan of a two-layer head");
+static_assert(ws_adjoint_plan<8>(1, 4, 8) && ws_adjoint_plan<16>(1, 4, 8) && ws_adjoint_plan<32>(1, 4, 8),
+              "adjoint plan of a one-layer head");
+
 template <int FT, bool GRAD, bool PROF>
 static int launch_wsq(QueryParams& p, cudaStream_t stream) {
-  const WsLayout lay = plan_ws_layout<FT>(p.dec, GRAD);
+  const WsLayout lay = plan_ws_layout<FT>(p.dec.n_hidden, p.dec.out_dim, GRAD);
   const size_t smem_bytes = (size_t)lay.total;
-  if (smem_bytes > 227 * 1024) {
+  if (smem_bytes > WS_SMEM_MAX) {
     set_error("wsq_decode kernel needs %zu B shared memory (> 227 KB)", smem_bytes);
     return PINB200_ERR_UNSUPPORTED;
   }

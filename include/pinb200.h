@@ -127,7 +127,7 @@ typedef struct pinb200_query_opts {
 #define PINB200_SPLIT_MIN_QUERIES 32768   /* decode-every-neighbour maps */
 #define PINB200_SPLIT_MIN_QUERIES_WF 1024 /* weighted_first maps whose decoder runs on the wgmma kernel (hidden 64, 1-2 layers,
                                              F in {8,16,32}): the two-launch pipeline is faster from ~1 k queries on */
-#define PINB200_SORT_MIN_QUERIES 131072
+#define PINB200_SORT_MIN_QUERIES 81920
 int64_t pinb200_query_workspace_bytes(int64_t n_queries);
 /* Run-time tunables of the query path (process-wide; for tests and A/B measurements):
      "split_min_queries"  batch size from which the two-launch pipeline is used, both kinds of map (<= 0 restores the

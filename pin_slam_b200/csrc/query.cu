@@ -27,7 +27,7 @@ namespace pinb {
 // K1a of the split pipeline: phase A1 alone, at high occupancy (no decoder weights in shared memory, <= 128
 // registers): the probe rounds of ~16 resident warps per SM keep the load/store unit busy, which the fused kernel's
 // 12 warps (most of them in compute phases at any time) cannot.  One warp = one 32-query tile.  COMPACT: the stash
-// blocks are StashS blocks (the decode runs on wsq_decode_kernel); with p.perm the tiles are runs of p.perm
+// blocks are StashS blocks (the decode runs on wsq_decode_kernel); with p.sorted the tiles are runs of p.sorted
 // (spatially sorted queries).
 template <bool SEEDS, bool COMPACT>
 __global__ void __launch_bounds__(128, 4) search_kernel(const __grid_constant__ QueryParams p) {
@@ -711,7 +711,7 @@ extern "C" int pinb200_query_sdf(const pinb200_map_view* map, const pinb200_deco
       char* base = static_cast<char*>(opts->workspace);
       const size_t used = (size_t)p.n_tiles * (StashS::floats + (want_seeds ? Seeds::floats : 0)) * sizeof(float);
       rc = sort_queries(query_xyz, opts->transform, n, map->resolution, base + used,
-                        (size_t)opts->workspace_bytes - used, &p.perm, (cudaStream_t)stream);
+                        (size_t)opts->workspace_bytes - used, &p.sorted, (cudaStream_t)stream);
       if (rc) return rc;
     }
     p.seeds = want_seeds ? p.stash + (size_t)p.n_tiles * StashS::floats : nullptr;

@@ -50,9 +50,10 @@ struct QueryParams {
   float* seeds;  // split pipeline with d/dq on the warp-specialised decode: [n_tiles][Seeds::floats] forward-mode seeds
   int pdl;       // host only: this decode launch directly follows its search launch (programmatic dependent launch)
   QueryLayout lay;
-  // search launch with spatially sorted queries (StashS blocks only): perm[i] = original index of the i-th query in
-  // sorted order; the search launch works on perm[32 st + lane].  nullptr: queries in the caller's order.
-  const int32_t* perm;
+  // search launch with spatially sorted queries (StashS blocks only): sorted[i] = {x, y, z, original index} of the
+  // i-th query in sorted order (the query untransformed); the search launch works on sorted[32 st + lane].  nullptr:
+  // queries in the caller's order.
+  const float4* sorted;
 };
 
 // squared distance with the reference's arithmetic: sum((p - q)^2) in fp32, no contraction (:990-994)
@@ -445,8 +446,8 @@ __device__ __forceinline__ void tangent_seeds(const pinb200_map_view& m, int K, 
     for (int i = 0; i < 3; ++i) sd[Seeds::P + (j * 3 + i) * WT + lane] = P[j][i];
 }
 
-// COMPACT: `stash` is a StashS block; with p.perm, lane `lane` works on query p.perm[q0s + lane] (per-query outputs
-// go to that index).  The seeds stay in tile order.
+// COMPACT: `stash` is a StashS block; with p.sorted, lane `lane` works on the query of record p.sorted[q0s + lane]
+// (per-query outputs go to its index).  The seeds stay in tile order.
 template <bool SEEDS = false, bool COMPACT = false>
 __device__ __forceinline__ void a1_tile(const QueryParams& p, const uint32_t* s_delta, long long q0s, int WQ, int lane,
                                         float* stash) {
@@ -463,18 +464,25 @@ __device__ __forceinline__ void a1_tile(const QueryParams& p, const uint32_t* s_
   float* s_pos = stash + (COMPACT ? StashS::pos : Stash::pos);
   const bool live = lane < WQ && q0s + lane < p.n;
   long long qi = q0s + lane;
+  float qx = 0.f, qy = 0.f, qz = 0.f;
   if (COMPACT) {
-    if (!live)
+    if (!live) {
       qi = -1;
-    else if (p.perm)
-      qi = __ldg(p.perm + q0s + lane);
+    } else if (p.sorted) {  // one coalesced 16-byte load: the query and its index
+      const float4 r = __ldg(p.sorted + q0s + lane);
+      qx = r.x;
+      qy = r.y;
+      qz = r.z;
+      qi = __float_as_int(r.w);
+    }
     reinterpret_cast<int*>(stash + StashS::perm)[lane] = (int)qi;
   }
-  float qx = 0.f, qy = 0.f, qz = 0.f;
   if (live) {
-    qx = __ldg(p.query_xyz + 3 * qi + 0);
-    qy = __ldg(p.query_xyz + 3 * qi + 1);
-    qz = __ldg(p.query_xyz + 3 * qi + 2);
+    if (!COMPACT || !p.sorted) {
+      qx = __ldg(p.query_xyz + 3 * qi + 0);
+      qy = __ldg(p.query_xyz + 3 * qi + 1);
+      qz = __ldg(p.query_xyz + 3 * qi + 2);
+    }
     if (p.opts.transform) {  // q = T p in fp32 (utils/tools.py:534-553)
       const double* T = p.opts.transform;
       const float x = fmaf(qz, (float)T[2], fmaf(qy, (float)T[1], qx * (float)T[0])) + (float)T[3];
@@ -630,6 +638,6 @@ int dispatch_wsq(QueryParams& p, cudaStream_t stream);
 void wsq_set_profile(int on);
 int wsq_read_profile(unsigned long long* host_out, int64_t count);
 int sort_queries(const float* xyz, const double* transform, long long n, float resolution, void* scratch,
-                 size_t scratch_bytes, const int32_t** perm, cudaStream_t stream);  // query_sort.cu
+                 size_t scratch_bytes, const float4** sorted, cudaStream_t stream);  // query_sort.cu
 
 }  // namespace pinb

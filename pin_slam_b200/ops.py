@@ -10,7 +10,7 @@ from ._lib import DecoderView, GnOpts, MapTrainOpts, MapView, QueryOpts, QueryOu
 
 SPLIT_MIN_QUERIES = 32768  # == PINB200_SPLIT_MIN_QUERIES (default; see set_option)
 SPLIT_MIN_QUERIES_WF = 1024  # == PINB200_SPLIT_MIN_QUERIES_WF: weighted_first maps on the tensor-core decode
-SORT_MIN_QUERIES = 131072  # == PINB200_SORT_MIN_QUERIES: spatial sort before the search launch (see set_option)
+SORT_MIN_QUERIES = 81920  # == PINB200_SORT_MIN_QUERIES: spatial sort before the search launch (see set_option)
 
 
 def uses_split(n: int, weighted_first: bool, dec=None, training_mode: bool = False) -> bool:

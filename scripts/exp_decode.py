@@ -7,8 +7,7 @@ decoder, d sdf / dq), the headline workload of bench.py:
   3. per-role cycle table of wsq_decode_kernel: per warp, clock deltas of the phases of its role, summed over one
      profiled launch (ws_profile); the role of every warp is read from the counters, so the table follows the kernel
 
-Section 2 counts the launches of the in-library spatial sort (histogram memset, sort_key_kernel, the scan's kernels,
-sort_scatter_kernel) with K1.
+Section 2 counts the two launches of the in-library spatial sort (sort_key_kernel, sort_scatter_kernel) with K1.
 With --presorted it also runs with the sort off (sort_min_queries 0), on the bench's random queries and on the same
 queries pre-permuted in Python into Morton order of their 0.4 m cells: the best that sorting inside the library
 could reach, without its cost.  --sort-sweep times K1 with the sort off and on over batch sizes (CUDA events, L2
@@ -111,7 +110,7 @@ def kernel_table(qq, label, trace_name):
     return out
 
 
-K1_KERNELS = ("search_kernel", "wsq_decode_kernel", "sort_key_kernel", "DeviceScan", "sort_scatter_kernel", "Memset")
+K1_KERNELS = ("search_kernel", "wsq_decode_kernel", "sort_key_kernel", "sort_scatter_kernel")
 out = kernel_table(q, "random queries, library defaults", "exp_decode_trace.json")
 if args.presorted:
     ops.set_option("sort_min_queries", 0)
@@ -120,7 +119,7 @@ if args.presorted:
     ops.set_option("sort_min_queries", ops.SORT_MIN_QUERIES)
 if args.sort_sweep:
     print("K1 cold-L2 time over batch sizes, sort off vs on (best of 3 alternating medians of 12 steps):")
-    for n in (1024, 2048, 4096, 8192, 16384, 32768, 65536, 200000):
+    for n in (1024, 2048, 4096, 8192, 16384, 32768, 65536, 81920, 100000, 131072, 200000):
         qn = q[:n].contiguous()
         o3 = {}
         res = {0: [], 1: []}

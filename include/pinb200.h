@@ -467,6 +467,29 @@ int pinb200_assemble_batch(const float* coord_pool, const float* label_pool, con
                            const int64_t* index, int64_t n, int32_t decimation, float eps, float* rows,
                            float* label, int32_t* ts, float* weight, float* color, void* stream);
 
+/* Mesh extraction (DESIGN.md row f5; utils/mesher.py:369-397 skimage marching cubes, :443-456 / :631 Open3D clean-up).
+   Grid: sdf fp32 / mask u8 (NULL: every cube) [nx*ny*nz], point p = (x*ny + y)*nz + z.  A corner is inside iff
+   sdf < level; cube (i,j,k) is polygonised iff mask at its lowest corner.  Vertex keys: 3*p + axis for the crossing of
+   the edge from grid point p along axis, at t = (level - a) / (b - a) (fp32); t exactly 0 or 1: 3*N + q for the grid
+   point q it lands on.  Triangles come in cube order, table order within a cube, degenerate ones (two equal keys)
+   dropped; right-hand normals point to sdf < level.
+   _count: number of triangles -> n_tri (device int64) and the per-block offsets -> scratch
+           (pinb200_mc_scratch_bytes(nx*ny*nz) bytes); _emit (same grid, same scratch): tri_keys [n_tri, 3] int64;
+   _vertices: grid-index-space positions pos [n_keys, 3] fp64 (i + t along the edge) of vertex keys.
+   pinb200_mesh_clusters: edge-connected triangle clusters.  edge_key [n_edges] ascending (one key per undirected
+   triangle edge), edge_tri [n_edges] the triangle of each, parent [n_tri] scratch; on return root [n_tri] holds the
+   smallest triangle id of each triangle's cluster and size [n_tri] the number of triangles of the cluster rooted there
+   (0 elsewhere). */
+int64_t pinb200_mc_scratch_bytes(int64_t n_points);
+int pinb200_mc_count(const float* sdf, const uint8_t* mask, int64_t nx, int64_t ny, int64_t nz, float level, void* scratch,
+                     int64_t* n_tri, void* stream);
+int pinb200_mc_emit(const float* sdf, const uint8_t* mask, int64_t nx, int64_t ny, int64_t nz, float level,
+                    const void* scratch, int64_t* tri_keys, void* stream);
+int pinb200_mc_vertices(const float* sdf, int64_t nx, int64_t ny, int64_t nz, float level, const int64_t* keys,
+                        int64_t n_keys, double* pos, void* stream);
+int pinb200_mesh_clusters(const int64_t* edge_key, const int32_t* edge_tri, int64_t n_edges, int64_t n_tri,
+                          int32_t* parent, int32_t* root, int32_t* size, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -131,6 +131,14 @@ SIGNATURES = {
     "pinb200_nccl_destroy": (C.c_int, [C.c_void_p]),
     "pinb200_color_loss": (C.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, C.c_int64, C.c_int32, C.c_float, C.c_int32,
                                      C.c_float, C.c_float, c_f32p, c_f32p, c_f32p, C.c_void_p]),
+    "pinb200_mc_scratch_bytes": (C.c_int64, [C.c_int64]),
+    "pinb200_mc_count": (C.c_int, [c_f32p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_float, C.c_void_p, C.c_void_p,
+                                   C.c_void_p]),
+    "pinb200_mc_emit": (C.c_int, [c_f32p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_float, C.c_void_p, C.c_void_p,
+                                  C.c_void_p]),
+    "pinb200_mc_vertices": (C.c_int, [c_f32p, C.c_int64, C.c_int64, C.c_int64, C.c_float, C.c_void_p, C.c_int64, c_f64p,
+                                      C.c_void_p]),
+    "pinb200_mesh_clusters": (C.c_int, [C.c_void_p, c_i32p, C.c_int64, C.c_int64, c_i32p, c_i32p, c_i32p, C.c_void_p]),
 }
 
 _lib = None

@@ -113,6 +113,13 @@ class HotPathConfig:
     dynamic_sdf_ratio_thre: float = 0.5
     dynamic_min_grad_norm_thre: float = 0.25
     pgo_on: bool = False
+    # mesh reconstruction (config.py:281-289)
+    mc_res_m: float = 0.3
+    pad_voxel: int = 3
+    skip_top_voxel: int = 2
+    mc_mask_on: bool = True
+    mesh_min_nn: int = 8
+    min_cluster_vertices: int = 300
 
     @property
     def infer_bs(self):

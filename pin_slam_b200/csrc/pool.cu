@@ -43,22 +43,9 @@ __global__ void __launch_bounds__(PF_TPB) pool_count_kernel(const float* __restr
   if (threadIdx.x == 0) bsum[blockIdx.x] = total;
 }
 
-__global__ void __launch_bounds__(1024) pool_scan_kernel(int* bsum, int n_blocks, long long n, long long n_tail,
-                                                         long long* counts) {
-  __shared__ int s_warp[64];
-  int carry = 0;
-  for (int base = 0; base < n_blocks; base += 1024) {
-    const int i = base + threadIdx.x;
-    const int v = i < n_blocks ? bsum[i] : 0;
-    int total;
-    const int ex = block_exclusive_scan(v, s_warp, total);
-    if (i < n_blocks) bsum[i] = carry + ex;
-    carry += total;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) counts[0] = carry;  // kept samples; counts[1] (kept among the last n_tail) is set by the scatter
-  (void)n;
-  (void)n_tail;
+__global__ void __launch_bounds__(1024) pool_scan_kernel(int* bsum, int n_blocks, long long* counts) {
+  const long long kept = scan_block_sums(bsum, bsum, n_blocks);
+  if (threadIdx.x == 0) counts[0] = kept;  // counts[1] (kept among the last n_tail) is set by the scatter
 }
 
 __global__ void __launch_bounds__(PF_TPB) pool_scatter_kernel(const PoolPtrs p, long long n, long long n_tail,
@@ -118,7 +105,7 @@ extern "C" int pinb200_pool_filter(const float* coord, const float* gcoord, cons
   PoolPtrs p{coord, gcoord, label, weight, color, ts, o_coord, o_gcoord, o_label, o_weight, o_color, o_ts, color_channels};
   cudaMemsetAsync(counts, 0, 16, st);
   pool_count_kernel<<<n_blocks, PF_TPB, 0, st>>>(gcoord, n, origin, radius2, scratch);
-  pool_scan_kernel<<<1, 1024, 0, st>>>(scratch, n_blocks, n, n_tail, (long long*)counts);
+  pool_scan_kernel<<<1, 1024, 0, st>>>(scratch, n_blocks, (long long*)counts);
   pool_scatter_kernel<<<n_blocks, PF_TPB, 0, st>>>(p, n, n_tail, origin, radius2, scratch, (long long*)counts);
   return check_launch("pool_filter");
 }

@@ -1,4 +1,5 @@
-// Block-wide exclusive prefix sum used by the compaction-style kernels (probe index, replay-pool filter, local map).
+// Block-wide exclusive prefix sum used by the compaction-style kernels (probe index, replay-pool filter, local map,
+// marching cubes).
 #pragma once
 #include "common.cuh"
 
@@ -31,5 +32,23 @@ __device__ __forceinline__ int block_exclusive_scan(int v, int* s_warp, int& tot
   return warp_off + inc - v;
 }
 
+// one block of blockDim.x (a multiple of 32, <= 1024) threads turns the per-block counts `in` [n_blocks] of a
+// count-then-scatter pair of kernels into exclusive offsets `out` (may alias `in`) and returns the grand total to every
+// thread; the running total is 64-bit, the partial sums of one pass over blockDim.x counts are not
+template <typename T>
+__device__ long long scan_block_sums(const int* in, T* out, int n_blocks) {
+  __shared__ int s_warp[64];
+  long long carry = 0;
+  for (int base = 0; base < n_blocks; base += blockDim.x) {
+    const int i = base + threadIdx.x;
+    const int v = i < n_blocks ? in[i] : 0;
+    int total;
+    const int ex = block_exclusive_scan(v, s_warp, total);
+    if (i < n_blocks) out[i] = (T)(carry + ex);
+    carry += total;
+    __syncthreads();
+  }
+  return carry;
+}
 
 }  // namespace pinb

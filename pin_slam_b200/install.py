@@ -9,12 +9,14 @@ import importlib
 import sys
 
 
-def install(tracker_and_mapper: bool = False) -> None:
+def install(tracker_and_mapper: bool = False, mesher: bool = False) -> None:
     """Register the drop-in `model.neural_points` / `model.decoder` modules.
 
     tracker_and_mapper=True additionally registers the fused `utils.tracker` / `utils.mapper` modules under the
     reference's names, so `from utils.tracker import Tracker` / `from utils.mapper import Mapper` in the reference
-    driver pick up the kernels' Tracker / Mapper (the other `utils.*` modules stay the reference's own)."""
+    driver pick up the kernels' Tracker / Mapper (the other `utils.*` modules stay the reference's own).
+    mesher=True registers the drop-in `utils.mesher` (marching cubes and mesh clean-up on the GPU; the reference's
+    module needs skimage and Open3D)."""
     np_mod = importlib.import_module("pin_slam_b200.model.neural_points")
     dec_mod = importlib.import_module("pin_slam_b200.model.decoder")
     sys.modules["model.neural_points"] = np_mod
@@ -30,3 +32,8 @@ def install(tracker_and_mapper: bool = False) -> None:
         if "utils" in sys.modules:
             sys.modules["utils"].tracker = trk
             sys.modules["utils"].mapper = mpr
+    if mesher:
+        msh = importlib.import_module("pin_slam_b200.utils.mesher")
+        sys.modules["utils.mesher"] = msh
+        if "utils" in sys.modules:
+            sys.modules["utils"].mesher = msh

@@ -596,3 +596,51 @@ def local_map_gather(points, orient, certainty, ts_update, local_mask, scratch, 
         _ptr(l_cert, torch.float32), _ptr(l_ts, torch.int32), _stream())
     _lib.check(rc, "pinb200_local_map_gather")
     _count()
+
+
+def _mc_grid(sdf: torch.Tensor, mask: Optional[torch.Tensor]):
+    if sdf.dim() != 3:
+        raise RuntimeError("marching cubes: sdf must be an [nx, ny, nz] grid")
+    if mask is not None and (mask.shape != sdf.shape or mask.dtype != torch.bool):
+        raise RuntimeError("marching cubes: mask must be a bool grid of the sdf's shape")
+    return _ptr(sdf, torch.float32), _ptr(mask), *[int(d) for d in sdf.shape]
+
+
+def mc_triangle_keys(sdf: torch.Tensor, mask: Optional[torch.Tensor], level: float = 0.0) -> torch.Tensor:
+    """pinb200_mc_count + pinb200_mc_emit: the marching-cubes triangles of the grid as vertex-key triples [T, 3] int64
+    (include/pinb200.h).  Reads the triangle count back to the host once to size the output."""
+    lib = _lib.load()
+    sp, mp, nx, ny, nz = _mc_grid(sdf, mask)
+    scratch = torch.empty(int(lib.pinb200_mc_scratch_bytes(sdf.numel())), dtype=torch.uint8, device=sdf.device)
+    n_tri = torch.empty(1, dtype=torch.int64, device=sdf.device)
+    _lib.check(lib.pinb200_mc_count(sp, mp, nx, ny, nz, float(level), scratch.data_ptr(), n_tri.data_ptr(), _stream()),
+               "pinb200_mc_count")
+    _count(2)
+    keys = torch.empty((int(n_tri.item()), 3), dtype=torch.int64, device=sdf.device)
+    if keys.shape[0]:
+        _lib.check(lib.pinb200_mc_emit(sp, mp, nx, ny, nz, float(level), scratch.data_ptr(), keys.data_ptr(), _stream()),
+                   "pinb200_mc_emit")
+        _count()
+    return keys
+
+
+def mc_vertices(sdf: torch.Tensor, keys: torch.Tensor, level: float = 0.0) -> torch.Tensor:
+    """pinb200_mc_vertices: grid-index-space positions [n, 3] float64 of the vertex keys [n] int64."""
+    sp, _, nx, ny, nz = _mc_grid(sdf, None)
+    pos = torch.empty((keys.shape[0], 3), dtype=torch.float64, device=sdf.device)
+    _lib.check(_lib.load().pinb200_mc_vertices(sp, nx, ny, nz, float(level), _ptr(keys, torch.int64), keys.shape[0],
+                                               pos.data_ptr(), _stream()), "pinb200_mc_vertices")
+    _count()
+    return pos
+
+
+def mesh_clusters(edge_key: torch.Tensor, edge_tri: torch.Tensor, n_tri: int):
+    """pinb200_mesh_clusters: (root [n_tri] int32 = smallest triangle id of each triangle's edge-connected cluster,
+    size [n_tri] int32 = triangles of the cluster rooted at that id) from the ascending undirected edge keys."""
+    parent, root, size = torch.empty((3, n_tri), dtype=torch.int32, device=edge_key.device).unbind(0)
+    _lib.check(_lib.load().pinb200_mesh_clusters(_ptr(edge_key, torch.int64), _ptr(edge_tri, torch.int32),
+                                                 edge_key.shape[0], int(n_tri), _ptr(parent), _ptr(root), _ptr(size),
+                                                 _stream()),
+               "pinb200_mesh_clusters")
+    _count(3)
+    return root, size

@@ -28,9 +28,21 @@ namespace pinb {
 // registers): the probe rounds of ~16 resident warps per SM keep the load/store unit busy, which the fused kernel's
 // 12 warps (most of them in compute phases at any time) cannot.  One warp = one 32-query tile.  COMPACT: the stash
 // blocks are StashS blocks (the decode runs on wsq_decode_kernel); with p.sorted the tiles are runs of p.sorted
-// (spatially sorted queries).
+// (spatially sorted queries).  A library built with -DPINB200_SEARCH_PROFILE=1 (csrc/build.sh takes extra nvcc flags)
+// stamps the phases of every tile (SearchClock); the default build has no profiling code in it.
+#ifndef PINB200_SEARCH_PROFILE
+#define PINB200_SEARCH_PROFILE 0
+#endif
+constexpr bool SEARCH_PROF = PINB200_SEARCH_PROFILE != 0;
+__device__ unsigned long long g_search_prof[SEARCH_PROF ? SEARCH_PROF_WARPS * SEARCH_PROF_SLOTS : 1];
+
+// Word rounds of 16 probes (the fused kernel keeps 32) hold half the word results in registers: the launch fits in
+// 128 registers without spilling, and 200 k sorted queries with d/dq search faster than with rounds of 32 (H100 SXM,
+// 700 W).  Rounds of 16 at 5 or 6 CTAs per SM (96 / 80 registers) spill to local memory and were slower.
+constexpr int SEARCH_CTAS_PER_SM = 4;  // 128-thread CTAs
+constexpr int SEARCH_SUPER = 16;       // probes per word round (knn_search_lane)
 template <bool SEEDS, bool COMPACT>
-__global__ void __launch_bounds__(128, 4) search_kernel(const __grid_constant__ QueryParams p) {
+__global__ void __launch_bounds__(128, SEARCH_CTAS_PER_SM) search_kernel(const __grid_constant__ QueryParams p) {
   extern __shared__ __align__(16) float smem[];
   uint32_t* s_delta = reinterpret_cast<uint32_t*>(smem);
   // programmatic dependent launch: the decode launch may start its prologue (mbarriers, weight staging) on the
@@ -39,9 +51,16 @@ __global__ void __launch_bounds__(128, 4) search_kernel(const __grid_constant__ 
   fill_probe_deltas(p.map, s_delta);
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
-  for (int st = blockIdx.x * nwarp + warp; st < p.n_tiles; st += gridDim.x * nwarp)
-    a1_tile<SEEDS, COMPACT>(p, s_delta, (long long)st * WT, WT, lane,
-                            p.stash + (size_t)st * (COMPACT ? StashS::floats : Stash::floats));
+  SearchClock<SEARCH_PROF> clk;
+  clk.start();
+  for (int st = blockIdx.x * nwarp + warp; st < p.n_tiles; st += gridDim.x * nwarp) {
+    clk.tile();
+    a1_tile<SEEDS, COMPACT, SEARCH_PROF, SEARCH_SUPER>(p, s_delta, (long long)st * WT, WT, lane,
+                                         p.stash + (size_t)st * (COMPACT ? StashS::floats : Stash::floats), clk);
+    clk.add(SP_TILES, 1u);
+  }
+  const int gw = blockIdx.x * nwarp + warp;
+  if (SEARCH_PROF && lane == 0 && gw < SEARCH_PROF_WARPS) clk.flush(g_search_prof + (size_t)gw * SEARCH_PROF_SLOTS);
 }
 
 // ---------------------------------------------------------------------------
@@ -107,7 +126,8 @@ __global__ void __launch_bounds__(WPB * 32, 1) query_kernel(const __grid_constan
       for (int i = 0; i < Stash::floats / 128; ++i) dst[i * 32 + lane] = t[i];
       __syncwarp();
     } else {
-      a1_tile(p, s_delta, q0s, WQ, lane, wsm + WL::stash);
+      SearchClock<false> clk;
+      a1_tile(p, s_delta, q0s, WQ, lane, wsm + WL::stash, clk);
     }
     if (WF) {  // the position part of the IDW-averaged decoder input (this thread's tile row) + zero padding
       s_x[lane * LDX + F + 0] = s_pos[0 * WT + lane];
@@ -610,8 +630,17 @@ static int launch_search(QueryParams& p, bool compact, cudaStream_t stream) {
   p.qpt = WT;
   p.n_tiles = (int)((p.n + WT - 1) / WT);
   const long long ctas = (p.n_tiles + 3) / 4;
-  const int grid = (int)std::min<long long>(ctas, (long long)sm_count() * 4);
+  const int grid = (int)std::min<long long>(ctas, (long long)sm_count() * SEARCH_CTAS_PER_SM);
   const size_t smem = align4(p.map.n_probe) * sizeof(float);
+  if (SEARCH_PROF) {  // warps of a smaller grid leave their counters zero
+    void* prof = nullptr;
+    cudaError_t e = cudaGetSymbolAddress(&prof, g_search_prof);
+    if (e == cudaSuccess) e = cudaMemsetAsync(prof, 0, sizeof(g_search_prof), stream);
+    if (e != cudaSuccess) {
+      set_error("search_profile: %s", cudaGetErrorString(e));
+      return PINB200_ERR_CUDA;
+    }
+  }
   if (!compact)
     search_kernel<false, false><<<grid, 128, smem, stream>>>(p);
   else if (p.seeds)
@@ -741,6 +770,23 @@ extern "C" int pinb200_query_sdf(const pinb200_map_view* map, const pinb200_deco
 
 extern "C" int pinb200_debug_read(const char* what, void* host_out, int64_t count) {
   if (what && std::string(what) == "ws_profile") return wsq_read_profile(reinterpret_cast<unsigned long long*>(host_out), count);
+  if (what && std::string(what) == "search_profile") {  // [SEARCH_PROF_WARPS][SEARCH_PROF_SLOTS] uint64, last launch
+    if (!SEARCH_PROF) {
+      set_error("search_profile: the library was built without -DPINB200_SEARCH_PROFILE=1");
+      return PINB200_ERR_UNSUPPORTED;
+    }
+    const int64_t have = SEARCH_PROF_WARPS * SEARCH_PROF_SLOTS;
+    if (count < have) {
+      set_error("search_profile: buffer of %lld < %lld counters", (long long)count, (long long)have);
+      return PINB200_ERR_BAD_ARG;
+    }
+    const cudaError_t e = cudaMemcpyFromSymbol(host_out, g_search_prof, sizeof(g_search_prof));
+    if (e != cudaSuccess) {
+      set_error("search_profile: %s", cudaGetErrorString(e));
+      return PINB200_ERR_CUDA;
+    }
+    return PINB200_OK;
+  }
   set_error("debug_read: unknown item '%s'", what ? what : "(null)");
   return PINB200_ERR_BAD_ARG;
 }

@@ -70,20 +70,62 @@ __device__ __forceinline__ uint32_t probe_slot(uint32_t r0, uint32_t delta, uint
 
 // ---------------------------------------------------------------------------
 // A1: thread-per-query search over the probe index (pinb200_map_view.probe_words / probe_rec).  Returns nn_count;
-// T holds the 8 best (distance, record rank) pairs, ascending.  Per 32 probes: one round of 8-byte word loads
+// T holds the 8 best (distance, record rank) pairs, ascending.  Per SUPER probes: one round of 8-byte word loads
 // (occupancy + rank), then the records of the occupied slots 16 at a time (two sorting-network batches per round
 // trip).  The odd last probe of an 8n+1 neighbourhood (33, 57, 81) is issued with the first round and inserted last.
 // ---------------------------------------------------------------------------
 constexpr int PROBE_SUPER = 32;
 constexpr int PROBE_ROUND = 16;
 
+// Optional cycle accounting of the search launch (a library built with -DPINB200_SEARCH_PROFILE=1): per warp, clock deltas of
+// the phases of a1_tile summed over the warp's tiles, for the first SEARCH_PROF_WARPS warps of the grid; read back with
+// pinb200_debug_read("search_profile", ...).  A stamp is taken when the warp issues the phase's last instruction, so
+// a load's latency counts in the phase that first uses its result.  Slots: the phases SP_HASH .. SP_OUT, the number of
+// distinct base slots (map voxels, up to hash collisions) of each tile summed over the warp's tiles, its tiles.
+enum SearchPhase { SP_HASH = 0, SP_WORDS, SP_SELECT, SP_WINNERS, SP_STASH, SP_OUT, SP_VOXELS, SP_TILES };
+constexpr int SEARCH_PROF_SLOTS = 8;
+constexpr int SEARCH_PROF_WARPS = 132 * 4 * 4;  // every warp of a full-size search grid on an H100 SXM
+template <bool PROF>
+struct SearchClock {  // PROF = false: no code at all
+  unsigned int acc[SEARCH_PROF_SLOTS];
+  unsigned int last;
+  __device__ __forceinline__ void start() {
+    if (PROF) {
+#pragma unroll
+      for (int i = 0; i < SEARCH_PROF_SLOTS; ++i) acc[i] = 0u;
+    }
+  }
+  __device__ __forceinline__ void tile() {
+    if (PROF) last = (unsigned int)clock();
+  }
+  __device__ __forceinline__ void lap(int slot) {
+    if (PROF) {
+      const unsigned int now = (unsigned int)clock();
+      acc[slot] += now - last;
+      last = now;
+    }
+  }
+  __device__ __forceinline__ void add(int slot, unsigned int v) {
+    if (PROF) acc[slot] += v;
+  }
+  __device__ __forceinline__ void flush(unsigned long long* dst) {
+    if (PROF) {
+#pragma unroll
+      for (int i = 0; i < SEARCH_PROF_SLOTS; ++i) dst[i] = acc[i];
+    }
+  }
+};
+
 __device__ __forceinline__ int probe_rank(uint2 w, uint32_t slot) {
   const uint32_t b = slot & 31u;
   return ((w.x >> b) & 1u) ? (int)(w.y + __popc(w.x & ((1u << b) - 1u))) : -1;
 }
 
+// SUPER: probes per word round (a multiple of PROBE_ROUND).  The batches of 8 and the order they are merged in do not
+// depend on it, so neither does the result: a smaller SUPER only holds fewer word results in registers at a time.
+template <int SUPER, bool PROF>
 __device__ __forceinline__ int knn_search_lane(const pinb200_map_view& m, const uint32_t* s_delta, bool live, uint32_t r0,
-                                               float qx, float qy, float qz, KnnTop& T) {
+                                               float qx, float qy, float qz, KnnTop& T, SearchClock<PROF>& clk) {
   knn_top_init(T);
   int count = 0;
   const uint32_t B = (uint32_t)m.buffer_size;
@@ -100,14 +142,14 @@ __device__ __forceinline__ int knn_search_lane(const pinb200_map_view& m, const 
     rk_last = probe_rank(__ldg(words + (slot >> 5)), slot);
   }
 #pragma unroll 1
-  for (int c0 = 0; c0 < Cb; c0 += PROBE_SUPER) {
+  for (int c0 = 0; c0 < Cb; c0 += SUPER) {
     const int nb = Cb - c0;
-    int rk[PROBE_SUPER];
+    int rk[SUPER];
     {
-      uint32_t slot[PROBE_SUPER];
-      uint2 wv[PROBE_SUPER];
+      uint32_t slot[SUPER];
+      uint2 wv[SUPER];
 #pragma unroll
-      for (int j = 0; j < PROBE_SUPER; ++j) {
+      for (int j = 0; j < SUPER; ++j) {
         slot[j] = 0u;
         wv[j] = make_uint2(0u, 0u);
         if (live && j < nb) {
@@ -116,10 +158,11 @@ __device__ __forceinline__ int knn_search_lane(const pinb200_map_view& m, const 
         }
       }
 #pragma unroll
-      for (int j = 0; j < PROBE_SUPER; ++j) rk[j] = probe_rank(wv[j], slot[j]);
+      for (int j = 0; j < SUPER; ++j) rk[j] = probe_rank(wv[j], slot[j]);
     }
+    clk.lap(SP_WORDS);
 #pragma unroll
-    for (int h = 0; h < PROBE_SUPER / PROBE_ROUND; ++h) {
+    for (int h = 0; h < SUPER / PROBE_ROUND; ++h) {
       if (h * PROBE_ROUND < nb) {
         float4 r[PROBE_ROUND];
 #pragma unroll
@@ -158,6 +201,7 @@ __device__ __forceinline__ int knn_search_lane(const pinb200_map_view& m, const 
     count += ok ? 1 : 0;
     knn_top_insert1(T, ok ? dd : SEL_INVALID_D2, ok ? rk_last : -1);
   }
+  clk.lap(SP_SELECT);
   return count;
 }
 
@@ -448,9 +492,9 @@ __device__ __forceinline__ void tangent_seeds(const pinb200_map_view& m, int K, 
 
 // COMPACT: `stash` is a StashS block; with p.sorted, lane `lane` works on the query of record p.sorted[q0s + lane]
 // (per-query outputs go to its index).  The seeds stay in tile order.
-template <bool SEEDS = false, bool COMPACT = false>
+template <bool SEEDS = false, bool COMPACT = false, bool PROF = false, int SUPER = PROBE_SUPER>
 __device__ __forceinline__ void a1_tile(const QueryParams& p, const uint32_t* s_delta, long long q0s, int WQ, int lane,
-                                        float* stash) {
+                                        float* stash, SearchClock<PROF>& clk) {
   const pinb200_map_view& m = p.map;
   const int K = p.opts.nn_k;
   int* s_li = reinterpret_cast<int*>(stash + Stash::li);
@@ -525,8 +569,13 @@ __device__ __forceinline__ void a1_tile(const QueryParams& p, const uint32_t* s_
     }
   } else {
     const uint32_t r0 = base_slot(m, qx, qy, qz);
+    if (PROF) {  // lanes of a voxel share r0 (base slots are < 2^31)
+      const uint32_t same = __match_any_sync(FULL, live ? r0 : 0xffffffffu);
+      clk.add(SP_VOXELS, __popc(__ballot_sync(FULL, live && __ffs(same) - 1 == lane)));
+    }
+    clk.lap(SP_HASH);
     KnnTop T;
-    cnt = knn_search_lane(m, s_delta, live, r0, qx, qy, qz, T);
+    cnt = knn_search_lane<SUPER>(m, s_delta, live, r0, qx, qy, qz, T, clk);
     // re-read the winners (the probe loop kept only distance + record rank through the sorting networks)
     const float4* __restrict__ rec4 = reinterpret_cast<const float4*>(m.probe_rec);
     float4 r[KREG];
@@ -595,10 +644,12 @@ __device__ __forceinline__ void a1_tile(const QueryParams& p, const uint32_t* s_
     s_q[1 * WT + lane] = qy;
     s_q[2 * WT + lane] = qz;
   }
+  clk.lap(SP_WINNERS);
   s_pos[0 * WT + lane] = sx;  // position part of the IDW-averaged decoder input (weighted_first)
   s_pos[1 * WT + lane] = sy;
   s_pos[2 * WT + lane] = sz;
   if (SEEDS) tangent_seeds(m, K, lif, w, px, py, pz, qx, qy, qz, usum, cnt, p.seeds + (size_t)(q0s / WT) * Seeds::floats, lane);
+  clk.lap(SP_STASH);
   if (live && !p.is_color) {
     if (p.opts.training_mode && (p.opts.training_rows <= 0 || qi < p.opts.training_rows)) {
       // certainty scatter_add / ts amax (:685-710); invalid entries add 0 / max with 0 in the reference
@@ -628,6 +679,7 @@ __device__ __forceinline__ void a1_tile(const QueryParams& p, const uint32_t* s_
       p.out.xyz[3 * qi + 2] = qz;
     }
   }
+  clk.lap(SP_OUT);
 }
 
 

@@ -6,6 +6,8 @@ decoder, d sdf / dq), the headline workload of bench.py:
      goes to DIR/exp_decode_trace.json
   3. per-role cycle table of wsq_decode_kernel: per warp, clock deltas of the phases of its role, summed over one
      profiled launch (ws_profile); the role of every warp is read from the counters, so the table follows the kernel
+  4. phase table of search_kernel: per warp, clock deltas of the phases of its tiles, summed over one launch, and the
+     distinct map voxels per 32-query tile (needs a library built with csrc/build.sh -DPINB200_SEARCH_PROFILE=1)
 
 Section 2 counts the two launches of the in-library spatial sort (sort_key_kernel, sort_scatter_kernel) with K1.
 With --presorted it also runs with the sort off (sort_min_queries 0), on the bench's random queries and on the same
@@ -165,3 +167,25 @@ for code in sorted(set(role_of.tolist())):
     busy = 1.0 - sum(share[s] for s in waits)
     print("  share:   " + "  ".join(f"{100 * s:8.1f}%" for s in share) +
           f"   busy (not waiting on another role) {100 * busy:.1f}%", flush=True)
+
+# ---- 4. phase table of search_kernel (a library built with csrc/build.sh -DPINB200_SEARCH_PROFILE=1)
+PHASES = ["sorted record + hash", "word round", "record rounds + selection", "winners + IDW + certainty",
+          "seeds + stash stores", "per-query outputs"]
+S_WARPS, S_SLOTS = 132 * 4 * 4, 8
+npm.query_sdf(q, dec, out=out)
+torch.cuda.synchronize()
+sbuf = np.zeros(S_WARPS * S_SLOTS, dtype=np.uint64)
+if _lib.load().pinb200_debug_read(b"search_profile", sbuf.ctypes.data, sbuf.size) != 0:
+    print("search_kernel phase table: rebuild with pin_slam_b200/csrc/build.sh -DPINB200_SEARCH_PROFILE=1", flush=True)
+    sys.exit(0)
+sp = sbuf.reshape(S_WARPS, S_SLOTS).astype(np.float64)
+sp = sp[sp[:, 7] > 0]  # warps that ran tiles
+tiles = sp[:, 7].sum()
+per_tile = sp[:, :6].sum(axis=0) / tiles
+print(f"search_kernel phases, cycles per 32-query tile (mean over {int(tiles)} tiles of {sp.shape[0]} warps; a load's "
+      "latency counts in the phase that first uses it):")
+for name, c in zip(PHASES, per_tile):
+    print(f"  {name:28s} {c:9.0f}  {100 * c / per_tile.sum():5.1f} %")
+print(f"  {'total':28s} {per_tile.sum():9.0f}   longest warp {int(sp[:, :6].sum(axis=1).max())} cycles over "
+      f"{int(sp[np.argmax(sp[:, :6].sum(axis=1)), 7])} tiles")
+print(f"  distinct map voxels per tile: mean {sp[:, 6].sum() / tiles:.2f}", flush=True)

@@ -490,6 +490,24 @@ int pinb200_mc_vertices(const float* sdf, int64_t nx, int64_t ny, int64_t nz, fl
 int pinb200_mesh_clusters(const int64_t* edge_key, const int32_t* edge_tri, int64_t n_edges, int64_t n_tri,
                           int32_t* parent, int32_t* root, int32_t* size, void* stream);
 
+/* Frame preparation (DESIGN.md row f6).
+   pinb200_frame_crop replaces the gathers by the down-sampling index (dataset/slam_dataset.py:437-439), crop_frame
+   (:1229-1248) and intrinsic_correct (:1251-1270): row j = index[i] of points [n, cols] (cols 3..7, fp32; the columns
+   after xyz travel along) is kept iff min_range < r < max_range and min_z < z < max_z, r = |xyz| in fp32.  With
+   correction_deg != 0, a = (float)(correction_deg / 180 * pi), v = asin(z / r), vc = v + a, x and y scale by
+   cos(vc) / cos(v) and z = r sin(vc).  Survivors -> points_out [K, cols] and ts_out [K] (ts and ts_out both NULL or
+   both set) in index order; K -> n_kept (device int64).  scratch: ceil(m / 1024) int32.
+   pinb200_deskew replaces utils/tools.py:747-779 (roma.rotmat_slerp): in place on the xyz columns of n rows
+   `row_stride` floats apart, p <- exp(s log R) p + s t with s = (ts - min ts) / (max ts - min ts) - ts_mid, pose
+   T_last<-cur [4,4] fp32 row-major on the device, log R the shortest-arc rotation vector.  scratch: 2 floats.  No
+   host synchronisation. */
+int pinb200_frame_crop(const float* points, int64_t n, int32_t cols, const int64_t* index, int64_t m, const float* ts,
+                       float min_z, float max_z, float min_range, float max_range, double correction_deg,
+                       int32_t* scratch, int64_t scratch_len, int64_t* n_kept, float* points_out, float* ts_out,
+                       void* stream);
+int pinb200_deskew(float* points, int64_t n, int64_t row_stride, const float* ts, const float* pose, float ts_mid,
+                   float* scratch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -139,6 +139,10 @@ SIGNATURES = {
     "pinb200_mc_vertices": (C.c_int, [c_f32p, C.c_int64, C.c_int64, C.c_int64, C.c_float, C.c_void_p, C.c_int64, c_f64p,
                                       C.c_void_p]),
     "pinb200_mesh_clusters": (C.c_int, [C.c_void_p, c_i32p, C.c_int64, C.c_int64, c_i32p, c_i32p, c_i32p, C.c_void_p]),
+    "pinb200_frame_crop": (C.c_int, [c_f32p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, c_f32p, C.c_float, C.c_float,
+                                     C.c_float, C.c_float, C.c_double, c_i32p, C.c_int64, C.c_void_p, c_f32p, c_f32p,
+                                     C.c_void_p]),
+    "pinb200_deskew": (C.c_int, [c_f32p, C.c_int64, C.c_int64, c_f32p, c_f32p, C.c_float, c_f32p, C.c_void_p]),
 }
 
 _lib = None

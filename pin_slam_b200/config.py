@@ -120,6 +120,18 @@ class HotPathConfig:
     mc_mask_on: bool = True
     mesh_min_nn: int = 8
     min_cluster_vertices: int = 300
+    # frame preparation (config.py:48-68, :216)
+    deskew: bool = False
+    min_z: float = -5.0
+    max_z: float = 80.0
+    min_range: float = 2.5
+    adaptive_range_on: bool = False
+    kitti_correction_on: bool = False
+    correction_deg: float = 0.0
+    vox_down_m: float = 0.05
+    source_vox_down_m: float = 0.8
+    rand_downsample: bool = False
+    rand_down_r: float = 1.0
 
     @property
     def infer_bs(self):

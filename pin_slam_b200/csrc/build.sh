@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# Build libpinb200.so (sm_90a, H100) in-tree: every .cu (here and in the mesh/ module) is compiled to build/<name>.o when it (or any header) is newer,
+# Build libpinb200.so (sm_90a, H100) in-tree: every .cu (here and in the mesh/ and frame/ modules) is compiled to build/<name>.o when it (or any header) is newer,
 # then linked.  Usage: build.sh [extra nvcc flags]   (extra flags force a full rebuild)
 set -euo pipefail
 here="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
@@ -11,7 +11,7 @@ newest_hdr=$(ls -t "$here"/*.cuh "$here"/../../include/pinb200.h | head -1)
 log="$here/../build.log"
 : > "$log"
 pids=()
-for src in "$here"/*.cu "$here"/mesh/*.cu; do
+for src in "$here"/*.cu "$here"/mesh/*.cu "$here"/frame/*.cu; do
   o="$obj/$(basename "${src%.cu}").o"
   if [ ! -f "$o" ] || [ "$src" -nt "$o" ] || [ "$newest_hdr" -nt "$o" ]; then
     ( nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xptxas -v "$@" \

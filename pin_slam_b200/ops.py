@@ -11,6 +11,7 @@ from ._lib import DecoderView, GnOpts, MapTrainOpts, MapView, QueryOpts, QueryOu
 SPLIT_MIN_QUERIES = 32768  # == PINB200_SPLIT_MIN_QUERIES (default; see set_option)
 SPLIT_MIN_QUERIES_WF = 1024  # == PINB200_SPLIT_MIN_QUERIES_WF: weighted_first maps on the tensor-core decode
 SORT_MIN_QUERIES = 81920  # == PINB200_SORT_MIN_QUERIES: spatial sort before the search launch (see set_option)
+CROP_IPB = 1024  # == FP_IPB of csrc/frame/prep.cu: index entries per block of pinb200_frame_crop
 
 
 def uses_split(n: int, weighted_first: bool, dec=None, training_mode: bool = False) -> bool:
@@ -644,3 +645,49 @@ def mesh_clusters(edge_key: torch.Tensor, edge_tri: torch.Tensor, n_tri: int):
                "pinb200_mesh_clusters")
     _count(3)
     return root, size
+
+
+def frame_crop(points: torch.Tensor, index: torch.Tensor, ts: Optional[torch.Tensor], min_z: float, max_z: float,
+               min_range: float, max_range: float, correction_deg: float = 0.0):
+    """pinb200_frame_crop: points[index] and ts[index] cropped to min_range < |xyz| < max_range, min_z < z < max_z and,
+    with correction_deg != 0, intrinsically corrected (slam_dataset.py:437-439, crop_frame, intrinsic_correct).
+    Returns (points_out [K, C], ts_out [K] or None); reads K back to the host once."""
+    lib = _lib.load()
+    n, cols = points.shape
+    m, dev = index.shape[0], points.device
+    scratch = torch.empty(max(1, (m + CROP_IPB - 1) // CROP_IPB), dtype=torch.int32, device=dev)
+    n_kept = torch.empty(1, dtype=torch.int64, device=dev)
+    out = torch.empty((m, cols), dtype=torch.float32, device=dev)
+    ts_out = None if ts is None else torch.empty((m,), dtype=torch.float32, device=dev)
+    rc = lib.pinb200_frame_crop(_ptr(points, torch.float32), n, cols, _ptr(index, torch.int64), m, _ptr(ts, torch.float32),
+                                float(min_z), float(max_z), float(min_range), float(max_range), float(correction_deg),
+                                _ptr(scratch), scratch.numel(), n_kept.data_ptr(), _ptr(out), _ptr(ts_out), _stream())
+    _lib.check(rc, "pinb200_frame_crop")
+    _count(3 if m else 0)
+    k = int(n_kept.item())
+    return out[:k], None if ts_out is None else ts_out[:k]
+
+
+def deskew_(points: torch.Tensor, ts: torch.Tensor, pose: torch.Tensor, ts_mid: float = 0.5) -> torch.Tensor:
+    """pinb200_deskew, in place on points[:, :3] (rows may be strided, e.g. the view cloud[:, :3]):
+    p <- exp(s log R) p + s t, s = (ts - min ts) / (max ts - min ts) - ts_mid, pose = T_last<-cur [4, 4]
+    (utils/tools.py:747-779).  No host synchronisation.  Returns `points`."""
+    n = points.shape[0]
+    if points.dim() != 2 or points.shape[1] < 3 or points.stride(1) != 1 or points.dtype != torch.float32:
+        raise RuntimeError("deskew_: points must be float32 [n, >=3] rows with unit column stride")
+    if not points.is_cuda:
+        raise RuntimeError("pin_slam_b200: the hot path runs on CUDA tensors only (no CPU fallback)")
+    ts = ts.reshape(-1)
+    if ts.shape[0] != n:
+        raise RuntimeError(f"deskew_: {ts.shape[0]} timestamps for {n} points")
+    pose = pose.to(device=points.device, dtype=torch.float32).contiguous()
+    if pose.shape != (4, 4):
+        raise RuntimeError("deskew_: pose must be [4, 4]")
+    if n == 0:
+        return points
+    scratch = torch.empty(2, dtype=torch.float32, device=points.device)
+    rc = _lib.load().pinb200_deskew(points.data_ptr(), n, points.stride(0), _ptr(ts.contiguous(), torch.float32),
+                                    _ptr(pose, torch.float32), float(ts_mid), _ptr(scratch), _stream())
+    _lib.check(rc, "pinb200_deskew")
+    _count(2)
+    return points
